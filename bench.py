@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- ChatTS-14B decode tokens/s on B200 (BASELINE.json metric), with roofline, e2e and CPU baseline.
+"""bench.py -- ChatTS-14B decode tokens/s on H100 (BASELINE.json metric), with roofline, e2e and CPU baseline.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference]
 
@@ -7,13 +7,14 @@ One JSON line on stdout (rank 0).  A "step" is one decode step of the whole batc
 sequence) of ChatTS-14B (synthetic bf16 weights at the real shapes -- no checkpoint exists offline) after a
 prefill of prompts that each carry 8 series x 256 points (8 x (46 prefix ids + <ts> + 16 patch rows + <ts/>)
 + 64 prompt ids = 576 merged positions).  `value` = B*K / device time of K steps (CUDA events, inputs
-resident in HBM; the 28 GB weight stream is far larger than the 126 MB L2).  `e2e` = the same metric through
+resident in HBM; the 28 GB weight stream is far larger than the 50 MB L2).  `e2e` = the same metric through
 the public generate() call with HOST tensors (processor output on the CPU, H2D of ids/series, prefill, K new
 tokens streamed back D2H every step).  N>1: tensor parallel over N GPUs (strong scaling, total work fixed).
 At N=1 a guarded probe (two child runs of this script on 4 layers) decides whether the measured run uses the cluster-fused decode GEMMs:
 only if they reproduce the default path's greedy tokens for every batch, faster (probe_decode_variant; --no-probe skips it).
 """
 import argparse
+import gc
 import json
 import os
 import subprocess
@@ -35,7 +36,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def tensor_peak():
@@ -43,7 +44,7 @@ def tensor_peak():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["bf16_tflops"]), "measured (MEASURED_PEAKS.json, cuBLAS bf16 burst)"
-    return 1700.0, "fallback (B200_PROFILING.md)"
+    return 989.0, "H100 SXM data sheet (dense bf16)"
 
 
 def _event_timer(fn, reps):
@@ -64,7 +65,7 @@ def measure_attention(model, st, batch, ctx_len, prompt_len, hbm_peak, timer=_ev
     ALONE on the launching stream:
       * paged flash-decode at the benchmark batch / context, one launch per LAYER's cache (48 x 84 MB at b=32 >> L2, so every
         launch streams its K/V from HBM) -> GB/s against the HBM peak (GQA intensity nh/nkv flop/B: HBM-bound);
-      * tcgen05 prefill attention over batch x prompt_len positions (Q/K/V/O 0.28 GB > L2) -> causal-useful TFLOP/s
+      * prefill attention over batch x prompt_len positions (Q/K/V/O 0.28 GB > L2) -> causal-useful TFLOP/s
         (4 * S^2/2 * d * nh per sequence) against the measured bf16 tensor peak."""
     import math
     c, L = model.ctx, model.L
@@ -90,21 +91,12 @@ def measure_attention(model, st, batch, ctx_len, prompt_len, hbm_peak, timer=_ev
     us = timer(lambda i: c.attn_prefill(q, k, v, cu, batch, prompt_len, nh, nkv, d, scale, o), 8)
     flops = batch * 4.0 * (prompt_len * prompt_len / 2.0) * d * nh
     peak, src = tensor_peak()
-    out["prefill"] = {"kernel": "attn_prefill_tc5_kernel (tcgen05, single-pass online softmax, S/O in TMEM)" if d == 128 else "attn_prefill_kernel (HMMA)",
+    out["prefill"] = {"kernel": "attn_prefill_wgmma_kernel (wgmma, S/O in registers)" if d == 128 else "attn_prefill_kernel (HMMA)",
                       "bound": "tensor", "us_per_launch": us, "causal_flops": flops, "achieved_tflops": flops / (us * 1e-6) / 1e12,
-                      "frac": flops / (us * 1e-6) / 1e12 / peak, "peak_tflops": peak, "peak_source": src, "tokens": T,
-                      "tensor_pipe_active_pct_ncu": None}
+                      "frac": flops / (us * 1e-6) / 1e12 / peak, "peak_tflops": peak, "peak_source": src, "tokens": T}
     # ---- the same prefill shape through the attention kernels INSTALLED on the box (SURVEY.md 2.2 K8: "the kernel to beat"): a stated
     # comparison only -- library code, never on the product path.  Each candidate is optional (import / arch support may be missing).
     out["prefill"]["vs_installed"] = installed_attention(q, k, v, batch, prompt_len, nh, nkv, d, scale, flops, timer)
-    try:       # tensor-pipe utilisation of the same kernel from the committed `ncu --set full` capture (a profiler number, never a timing)
-        cap = json.load(open(os.path.join(ROOT, "profiles", "r1_ncu_summary.json")))
-        out["decode"]["dram_pct_of_peak_ncu"] = float(cap["decode_attention_b32_ctx576"][0]["dram_pct_of_peak"])
-        cap2 = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_attention_summary.json")))      # the single-pass kernel of round 2
-        out["prefill"]["tensor_pipe_active_pct_ncu"] = float(cap2["prefill_attention_tcgen05_b32x576"][0]["tensor_pipe_active_pct"])
-        out["ncu_source"] = "profiles/r1_ncu_summary.json (decode), profiles/r2_ncu_attention_summary.json (prefill)"
-    except Exception:
-        pass
     return out
 
 
@@ -176,7 +168,7 @@ def make_batch(cfg, batch, seed=0, n_series=N_SERIES, series_len=SERIES_LEN):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -334,7 +326,7 @@ def workload_config(batch, gpus):
                          f"each prompt {N_SERIES} series x {SERIES_LEN} points -> 576 merged positions "
                          f"({N_SERIES}x({PREFIX_IDS} prefix ids+<ts>+16 patch rows+<ts/>)+{PROMPT_IDS} prompt ids)"),
             "batch": batch, "context": 576, "parallelism": f"tp{gpus}" if gpus > 1 else "single-gpu",
-            "l2_policy": "inputs larger than L2: 28 GB of weights streamed per step vs 126 MB L2"}
+            "l2_policy": "inputs larger than L2: 28 GB of weights streamed per step vs 50 MB L2"}
 
 
 # ------------------------------------------------------------------------------------------------ decode-variant probe
@@ -459,7 +451,7 @@ def tp_parity_gate(world, rank, layers=4, batch=8, seed=77):
     dist.barrier()
     return out
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ native arm
 def measure_config4(cfg, rank, world, steps, warmup, sync_all, batch=8, n_series=30, series_len=512):
     """BASELINE.json configs[3]: batch-8 decode with 30 series x 512 points per prompt (30 x (46 prefix ids + <ts> + 32 patch rows + <ts/>)
     + 64 prompt ids = 2 464 merged positions), tensor-parallel over however many GPUs the run has (the config names 8).  A second model
@@ -662,11 +654,22 @@ def run_b200(args):
             ctx_end = int(lay.lens.max()) + n_tok
             import hashlib
             tok_sha = hashlib.sha1(st.out_tokens[:, :n_tok].to(torch.int32).cpu().numpy().tobytes()).hexdigest()[:16]
+            if args.dump_outputs and batch == args.batch:
+                # what a caller of the timed decode step receives: the last step's logits and the greedy tokens so far
+                logits = st.full_logits[:batch].float().cpu().numpy()
+                cap = (48 << 20) // (4 * logits.shape[1])                   # rows within ~48 MB, leaving room for the tokens
+                if batch > cap:                                             # a fixed, seeded sample of rows for large batches
+                    rows = np.sort(np.random.default_rng(0).choice(batch, cap, replace=False))
+                    logits = logits[rows]
+                    dumped["logits_rows"] = rows.astype(np.float64)
+                dumped["logits"] = logits
+                dumped["tokens"] = st.out_tokens[:batch, :n_tok].cpu().numpy().astype(np.float64)
         finally:
             model.pool.release(held)
         return ms, per_step_launches, ctx_end, tok_sha
 
     results = {}
+    dumped = {}
     with ClockSampler(local) as clk:
         batches = [args.batch] if args.only_batch else sorted(set(b for b in (1, 8, args.batch) if b <= args.batch))
         for b in batches:
@@ -675,6 +678,10 @@ def run_b200(args):
                               ctx_end=ctx_end)
     clocks = clk.summary()
     main = results[args.batch]
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dumped.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
 
     # ---- whole-step HBM roofline: streamed weights + KV read per step (SURVEY.md §8d)
     L = cfg.num_hidden_layers
@@ -686,7 +693,7 @@ def run_b200(args):
     step_bytes = w_bytes + args.batch * ctx_mid * kv_tok
     step_gbs = step_bytes / (main["ms_per_step"] / 1e3) / 1e9
 
-    # ---- dominant kernel alone: gate_up tcgen05 GEMM (2*I*H weights), one launch per layer weight so every launch
+    # ---- dominant kernel alone: gate_up wgmma GEMM (2*I*H weights), one launch per layer weight so every launch
     # streams a different 283 MB from HBM (>> L2), timed with CUDA events on the launching stream
     roof = None
     if world == 1:
@@ -715,12 +722,12 @@ def run_b200(args):
                 traffic = json.load(open(os.path.join(ROOT, "profiles", "r1_ncu_summary.json")))["gate_up_decode_traffic_bytes_per_launch"]
         except Exception:
             traffic = None
-        roof = {"bound": "hbm", "kernel": "gemm_tn_kernel (gate_up projection, tcgen05/TMA, swap-AB, split-K 2)", "achieved": ach, "peak": hbm_peak,
+        roof = {"bound": "hbm", "kernel": "gemm_tn_kernel (gate_up projection, wgmma/TMA, swap-AB, split-K)", "achieved": ach, "peak": hbm_peak,
                 "unit": "GB/s", "frac": ach / hbm_peak, "traffic": traffic, "us_per_launch": us, "algorithmic_bytes": alg,
                 "peak_source": peak_src, "split_k": sp,
                 "whole_step": {"bytes": step_bytes, "achieved_gbs": step_gbs, "frac": step_gbs / hbm_peak}}
         if getattr(model, "use_fused_decode", 0):
-            # the measured step ran the cluster-fused variant of this projection (same TMA -> tcgen05 mainloop per K split, reduction and
+            # the measured step ran the cluster-fused variant of this projection (same TMA -> wgmma mainloop per K split, reduction and
             # SwiGLU in the epilogue): time THAT kernel too, same weights, same algorithmic bytes
             try:
                 fs = min(sp, 8)
@@ -740,7 +747,7 @@ def run_b200(args):
                 roof["fused_variant"] = {"error": repr(e)[:200]}
 
     # ---- TS encoder alone (north_star: reported against the HBM roofline): N = 8*B series x 256 points -> 128*B patch rows,
-    # L2 flushed (256 MB write) before every timed call, CUDA events around the encode (patchify + 5 tcgen05 GEMM layers)
+    # L2 flushed (256 MB write) before every timed call, CUDA events around the encode (patchify + 5 wgmma GEMM layers)
     ts_roof = None
     if world == 1:
         def ts_case(nb):
@@ -816,6 +823,16 @@ def run_b200(args):
                              f"{args.batch}x576 positions and {new} decode steps with per-step D2H of the new ids; value = B*new/wall",
                "seconds": dt, "out_shape": list(out.shape)}
 
+    # The side blocks build model instances of their own: release this one first, so that each of them has the GPU's memory to itself
+    # (80 GB hold one 14B model with its KV pool and CUDA graphs, not two or three)
+    arch = ctx.arch
+    variants = {k: int(getattr(model, a, 0) or 0) for k, a in (("decode_fused", "use_fused_decode"), ("peer_ll", "use_peer_ll"),
+                                                               ("native_step", "use_native_step"), ("decode_chain", "use_chain"))}
+    st = None
+    del model, ctx
+    gc.collect()
+    torch.cuda.empty_cache()
+
     # ---- BASELINE.json configs[3] (batch-8 decode, 30 series x 512 points) on this run's GPUs: a side block, never fatal for the headline
     config4 = None
     if not args.sweep_only and not args.layers and not args.no_config4:
@@ -823,6 +840,8 @@ def run_b200(args):
             config4 = measure_config4(cfg, rank, world, args.steps, args.warmup, sync_all)
         except Exception as e:  # pragma: no cover
             config4 = {"error": repr(e)[:300]}              # shape / capacity errors are the same on every rank: all of them land here
+        gc.collect()
+        torch.cuda.empty_cache()
 
     # ---- GPTQ-Int4 side block (one GPU: W4A16 decode weights are single-GPU)
     w4_block = None
@@ -844,7 +863,7 @@ def run_b200(args):
                 "vs_baseline": None, "dtype": "bf16", "data": "synthetic", "config": workload_config(args.batch, world),
                 "by_batch": {str(b): {"tokens_per_s": r["tokens_per_s"], "ms_per_step": r["ms_per_step"], "tokens_sha1": r.get("tokens_sha1")} for b, r in results.items()},
                 "clocks": clocks, "e2e": e2e, "gpu_launches": int(main["launches"] * args.steps), "launches_per_step": main["launches"],
-                "roofline": roof, "ts_encoder": ts_roof, "attention": attn_roof, "cpu_baseline": cpu, "arch": ctx.arch, "lib": os.path.relpath(_cabi.LIB_PATH, ROOT)}
+                "roofline": roof, "ts_encoder": ts_roof, "attention": attn_roof, "cpu_baseline": cpu, "arch": arch, "lib": os.path.relpath(_cabi.LIB_PATH, ROOT)}
         # which opt-in variants of the decode path this line was measured with (all off = the validated default path)
         line["config4"] = config4
         line["w4a16"] = w4_block
@@ -857,8 +876,7 @@ def run_b200(args):
             # reduce-scatter of fp32 pairs (8 B on the wire per element incl. epochs) to the owners + all-gather of the rounded h
             # (4 B per element incl. epochs), (world-1)/world of it leaving the GPU
             line["nvlink_bytes_per_step_per_rank"] = int(2 * L * args.batch * cfg.hidden_size * 12 * (world - 1) / world)
-        line["config"]["variants"] = {k: int(getattr(model, a, 0) or 0) for k, a in (("decode_fused", "use_fused_decode"), ("peer_ll", "use_peer_ll"),
-                                                                                   ("native_step", "use_native_step"), ("decode_chain", "use_chain"))}
+        line["config"]["variants"] = variants
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.barrier()
@@ -880,8 +898,9 @@ def main():
     ap.add_argument("--no-w4", action="store_true", help="skip the GPTQ-Int4 side block (third model instance with 4-bit projections)")
     ap.add_argument("--no-config4", action="store_true", help="skip the BASELINE configs[3] side block (second model instance, 30 x 512-point prompts)")
     ap.add_argument("--no-probe", action="store_true", help="(default) the default decode path is measured as is")
-    ap.add_argument("--probe", action="store_true", help="guarded child-process probe of the cluster-fused decode variants (round 1; measured slower at b = 32 on a B200, "
-                                                        "profiles/r2_decode_variants_ab.txt, so no longer on by default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed decode steps of --batch, write their outputs (last-step logits, greedy tokens) as DIR/<name>.npy")
+    ap.add_argument("--probe", action="store_true", help="guarded child-process probe of the cluster-fused decode variants (opt-in)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":

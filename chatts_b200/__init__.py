@@ -1,8 +1,8 @@
-"""chatts_b200 -- B200-native (sm_100a) hot path of ChatTS: the Value-Preserved Time-Series Encoder and the
+"""chatts_b200 -- H100-native (sm_90a) hot path of ChatTS: the Value-Preserved Time-Series Encoder and the
 Qwen2 decoder forward behind the reference's processor / ``<ts>`` protocol / generate() surface.
 
 Importing the package is GPU-free (config, layout, processor are host logic); anything that computes goes through
-libchatts_b200.so and raises if the library or a B200 is missing -- there is no fallback path."""
+libchatts_b200.so and raises if the library or an H100 is missing -- there is no fallback path."""
 from .config import ChatTSConfig
 from .processor import ChatTSProcessor, SimpleTokenizer, sp_encoding
 

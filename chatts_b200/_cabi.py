@@ -1,7 +1,7 @@
 """ctypes binding of libchatts_b200.so (include/chatts_b200.h).
 
 This is the ONLY compute path of the package: there is no Python / torch fallback behind any wrapper, and
-importing the package on a machine where the library is missing or where no sm_100 GPU is visible raises
+importing the package on a machine where the library is missing or where no sm_90 GPU is visible raises
 as soon as a kernel is requested.  torch is used for device memory, streams and torch.distributed only.
 """
 import ctypes as C
@@ -119,7 +119,7 @@ def load_library():
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise CtsError(f"{LIB_PATH} is missing: run `python -m chatts_b200.build` (nvcc, sm_100a). "
+        raise CtsError(f"{LIB_PATH} is missing: run `python -m chatts_b200.build` (nvcc, sm_90a). "
                        "chatts_b200 has no CPU or torch fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, i, ll, f = C.c_void_p, C.c_int, C.c_longlong, C.c_float
@@ -212,7 +212,7 @@ def dtype_code(dt):
         return BF16
     if dt == torch.float16:
         return F16
-    raise CtsError(f"unsupported model dtype {dt}: the sm_100a kernels compute in bf16 or fp16 with fp32 accumulate")
+    raise CtsError(f"unsupported model dtype {dt}: the sm_90a kernels compute in bf16 or fp16 with fp32 accumulate")
 
 
 def _p(t):
@@ -224,17 +224,17 @@ def _stream():
 
 
 class Context:
-    """One per (process, device).  Raises if the GPU is not sm_100 -- there is nothing else to run on."""
+    """One per (process, device).  Raises if the GPU is not sm_90 -- there is nothing else to run on."""
 
     def __init__(self, device=None):
         if not torch.cuda.is_available():
-            raise CtsError("no CUDA device visible: chatts_b200 runs on B200 (sm_100a) only, with no CPU fallback")
+            raise CtsError("no CUDA device visible: chatts_b200 runs on H100 (sm_90a) only, with no CPU fallback")
         self.lib = load_library()
         self.device = torch.cuda.current_device() if device is None else torch.device(device).index or 0
         h = C.c_void_p()
         rc = self.lib.cts_ctx_create(self.device, C.byref(h))
         if rc != OK or not h:
-            raise CtsError(f"cts_ctx_create(device={self.device}) failed with {rc} (needs an sm_100 device)")
+            raise CtsError(f"cts_ctx_create(device={self.device}) failed with {rc} (needs an sm_90 device)")
         self.h = h
         self.arch = self.lib.cts_arch().decode()
         self.launches = 0          # kernels launched through this ctx (bench.py's gpu_launches evidence)

@@ -1,9 +1,9 @@
-"""Build libchatts_b200.so (hand-written sm_100a CUDA + the C-ABI) in-tree with nvcc.
+"""Build libchatts_b200.so (hand-written sm_90a CUDA + the C-ABI) in-tree with nvcc.
 
     python -m chatts_b200.build          # incremental
     python -m chatts_b200.build --force
 
-nvcc cross-compiles without a GPU; the .so lands in chatts_b200/lib/ (git-ignored, shipped to the GPU box).
+nvcc cross-compiles without a GPU; the .so lands in chatts_b200/lib/ (git-ignored).
 """
 import os
 import subprocess
@@ -16,11 +16,12 @@ OBJ = os.path.join(CSRC, "_build")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libchatts_b200.so")
 SOURCES = ["ctx.cu", "gemm_tcgen05.cu", "ts_frontend.cu", "elementwise.cu", "attention.cu", "allreduce.cu", "decode_chain.cu",
-           "train_elementwise.cu", "attention_bwd.cu", "sampling.cu", "decoder_step.cu", "attention_bwd_tc5.cu", "lora_wgrad_mma.cu", "gemm_decode_fused.cu", "allreduce_ll.cu", "ts_encoder_fused.cu", "gemm_w4.cu", "gemm_w4_mma.cu"]
+           "train_elementwise.cu", "attention_bwd.cu", "attention_bwd_wgmma.cu", "sampling.cu", "decoder_step.cu", "lora_wgrad_mma.cu", "gemm_decode_fused.cu", "allreduce_ll.cu", "ts_encoder_fused.cu", "gemm_w4.cu", "gemm_w4_mma.cu"]
 HEADERS = ["common.cuh", "tensormap.cuh", "trace.cuh", "ts_rows.cuh", os.path.join("..", "..", "include", "chatts_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
-         '-DCTS_BUILD_ARCH="sm_100a"', "-diag-suppress", "177"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+         '-DCTS_BUILD_ARCH="sm_90a"', "-diag-suppress", "177"]
 
 
 def _newer(src_list, target):
@@ -57,7 +58,7 @@ def build(force=False, verbose=True):
                 raise RuntimeError(f"nvcc failed on {src}")
     objs = [os.path.join(OBJ, s.replace(".cu", ".o")) for s in srcs]
     if force or jobs or _newer(objs, LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ARCH
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)

@@ -32,7 +32,7 @@ class ChatTSConfig:
     eos_token_id: int = 151645                  # stop ids 151643/151645 (chatts/utils/llm_utils.py:153)
     pad_token_id: int = 151643
     # HF-surface merge of the patch rows at <ts><ts/> (layout.py): "insert" keeps both special tokens, "overwrite" replaces the pair.
-    # The checkpoint's remote code is not in the reference repo, so this cannot be pinned offline (DESIGN.md §2, INTEGRATION.md).
+    # The checkpoint's remote code is not in the reference repo, so this cannot be pinned offline (INTEGRATION.md).
     ts_merge_mode: str = "insert"
     model_type: str = "chatts"                  # scripts/start_vllm_server.sh:5
     torch_dtype: str = "bfloat16"

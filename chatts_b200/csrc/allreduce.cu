@@ -9,7 +9,7 @@
 // local slots in rank order -- the same order on every rank, so all ranks hold bit-identical h without a broadcast --
 // fused with the residual add and the next RMSNorm.  No NCCL call, no extra launch, no copy.  (allreduce_ll.cu is the
 // two-shot variant with the flags inside the data.)  The two partial buffers (o_proj / down_proj) alternate, so
-// the barrier of call n+1 is what licenses overwriting the buffer of call n (see DESIGN.md).
+// the barrier of call n+1 is what licenses overwriting the buffer of call n.
 #include <cooperative_groups.h>
 
 #include "common.cuh"

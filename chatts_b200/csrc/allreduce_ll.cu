@@ -5,8 +5,7 @@
 //     h = resid + dtype( sum over ranks of partial_r ) ;  norm_out = RMSNorm(h) * w          (vllm qwen2.py:100-116,168-174)
 //
 // The one-shot kernel of allreduce.cu pushes every rank's full fp32 partial to every rank ((W-1) x T x H x 4 bytes of NVLink
-// egress per call, ordered by fence + release flag + acquire poll).  Measured at TP8 (profiles/r1_bench_tp8.json) the decode
-// step spends most of its 6.6 ms in those 96 calls.  Here, per call and token:
+// egress per call, ordered by fence + release flag + acquire poll); at TP8 those calls dominate the decode step.  Here, per call and token:
 //   phase A  each rank sums its split-K partials and SCATTERS: columns of owner j go to rank j          (reduce-scatter, fp32)
 //   phase B  the owner waits for the W contributions of its columns (polling the epoch words of the data itself), adds them in
 //            RANK ORDER, adds the residual, rounds -> its H/W columns of h, plus the sum of squares of those columns; it

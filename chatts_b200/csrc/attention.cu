@@ -4,8 +4,8 @@
 //  cts_attn_prefill : variable-length causal attention over the tokens of one call (no prefix).  Tensor-core
 //                     (HMMA via nvcuda::wmma) flash attention in two passes over the KV tiles: pass 1 finds the
 //                     row max / row sum, pass 2 accumulates exp(s - m) V in fragments, so no accumulator rescale
-//                     is needed.  Round-1 kernel: prefill attention is ~1% of the prefill FLOPs at the benchmark
-//                     prompt (576 tokens); the tcgen05/TMEM version is the round-2 item in DESIGN.md.
+//                     is needed; head_dim 64.  head_dim 128 runs attn_prefill_wgmma_kernel (wgmma, single-pass online
+//                     softmax with S and O in registers).
 //  cts_attn_decode  : one query token per sequence against the PAGED KV cache, flash-decoding split over pages.
 //                     HBM-bound (GQA intensity = nh/nkv flop/B): K/V pages are pulled with cp.async.bulk into a
 //                     double-buffered shared-memory ring (mbarrier complete_tx), all q heads of a kv head share
@@ -236,353 +236,164 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
 }
 
 // ================================================================================================
-// prefill on tcgen05 (head_dim 128): S = Q K^T and O += P V on the 5th-gen tensor cores, accumulators in TMEM
+// prefill on wgmma (head_dim 128): one CTA = 64 query rows of one (sequence, head).  Warp 4 streams Q once and the K/V tiles
+// of the causal range through a two-stage TMA ring (128-byte swizzle, two 64-column halves per 128-wide row); warps 0..3 are
+// one warpgroup that computes S[64 x 64] = Q K^T with wgmma (both operands K-major in shared memory), runs the online softmax
+// on the S registers (thread = two query rows, a quad of lanes shares a row), and accumulates O[64 x 128] += P V with P fed
+// straight from registers as the A operand and V as the MN-major B operand.  S and O never leave the registers; the epilogue
+// writes O / l (and the log-sum-exp for the backward).
 // ================================================================================================
-// One CTA = 128 query rows of one (sequence, head).  Q, K, V tiles arrive by TMA (128-byte swizzle); the MMA warp
-// issues tcgen05.mma (M=128, N=64, K=16) for S[128 x 64] = Q K^T into one of two TMEM buffers; the four softmax warps
-// (thread = query row, lane-aligned with TMEM) read S with tcgen05.ld and run a SINGLE-PASS online softmax:
-//   * the row maximum used for the exponent is refreshed lazily -- only when the tile's maximum exceeds it by more than 8
-//     (in log2 units; P then stays below 2^8, far inside bf16 / fp16 / fp32 range) -- so the O accumulator in TMEM needs a
-//     rescale only in the first tiles of a row block; when any row of a warp needs one, the warp multiplies its 32 TMEM
-//     lanes of O in place (tcgen05.ld -> scale -> tcgen05.st) between P.V of the previous tile and P.V of this one;
-//   * P = exp2(s * scale*log2e - m) as bf16/fp16 into a swizzled K-major shared tile, the row sum kept in fp32, and the
-//     MMA warp issues O[128 x 128] += P V into TMEM columns 128..255 (V is the MN-major B operand).
-// Round 1-2 ran two passes (row maxima first, so that O never needed a rescale): 1.5 x the tensor work and twice the
-// TMEM reads of S per tile; 254 TFLOP/s at 32 x 576 (profiles/r2_prefill_attention_vs_installed.json).  Causal masking
-// only touches the tiles on the diagonal (query tiles are 128, key tiles 64, both aligned).  Epilogue: O / l from TMEM to global.
-constexpr int kTcQ = 128, kTcKV = 64, kTcThreads = 192;
-constexpr int kTcQHalf = kTcQ * 128;            // one [128 q rows x 128 B] swizzled half of the Q tile (16 KiB)
-constexpr int kTcKHalf = kTcKV * 128;           // one [64 kv rows x 128 B] half of a K or V tile (8 KiB)
-constexpr int kTcStages = 3;                    // K/V ring: tiles of 2 x 8 KiB, consumed in the order they are loaded
-constexpr int kTcSmem = 2 * kTcQHalf + kTcQ * 128 + kTcStages * 2 * kTcKHalf;   // Q 32 + P 16 + ring 48 = 96 KiB -> 2 CTAs / SM
+constexpr int kWgQ = 64, kWgKV = 64, kWgStages = 2, kWgThreads = 160;
+template <typename T> __device__ __forceinline__ uint32_t pack2(float lo, float hi);   // defined with the decode kernel below
+constexpr int kWgHalf = 64 * 128;                         // one [64 rows x 128 B] swizzled half of a Q, K or V tile (8 KiB)
+constexpr int kWgStageBytes = 4 * kWgHalf;                // K and V tile
+constexpr int kWgSmem = 2 * kWgHalf + kWgStages * kWgStageBytes;
 
-// MN-major (N contiguous) B operand, 128B swizzle: atoms of [8 K-rows x 64 N-elements]; LBO = stride between the
-// 64-element N atoms (the two d-halves of the V tile), SBO = stride between consecutive 8-row K groups.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)(lbo_bytes >> 4) << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Pipeline (per CTA; two CTAs share an SM): K and V tiles travel through ONE ring of kTcStages slots in exactly the order the MMA
-// warp consumes them (K_0, K_1, V_0, K_2, V_1, ..., V_{n-1}), so the TMA producer runs up to three tiles ahead; S is double-buffered
-// in TMEM (2 x 64 columns) and the MMA warp issues QK^T of tile i BEFORE P.V of tile i-1, so the softmax warps work on tile i while
-// the tensor core runs P.V(i-1); P is single-buffered behind a p_free barrier, which is also what orders an O rescale (done by the
-// softmax warps after p_free = "P.V(i-1) has completed" and before their p_full arrival = "P.V(i) may be issued").
-// 2^x on the MUFU (ex2.approx.ftz: relative error 2^-22, flushes denormal results -- P values that small do not matter); exp2f()
-// without fast-math wraps the same instruction in a denormal range fix-up of three more
-__device__ __forceinline__ float tc_ex2(float x) {
-#ifndef CTS_HOST_SHIM
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-#else
-  return exp2f(x);
-#endif
-}
-
-// Persistent CTAs (two per SM) over the (query tile, head, sequence) work items, heaviest query tiles first: at the benchmark shape an
-// item is 2..9 key tiles, and with one CTA per item (round 2's first single-pass version) barrier set-up, the 256-column TMEM
-// allocation, the first Q / K round trips and the O epilogue were ~45 % of a CTA's life.  Here the pipeline state simply carries on
-// from item to item: the producer requests the next item's Q as soon as the last QK^T of the current one has completed (q_free) and its
-// K tiles as ring slots free up; the MMA warp starts the next item's QK^T while the softmax warps still store the current O, and only
-// the first P.V of an item waits for those warps to have read O (o_free).
-struct TcItem {
-  int seq0, len, q0, head, kvh, nt;
-};
-__device__ __forceinline__ bool tc_item(int idx, int nqt, int nh, int nkv, int batch, const int* __restrict__ cu_seqlens, TcItem& it) {
-  const int per_qt = nh * batch;
-  const int qt = nqt - 1 - idx / per_qt;              // long rows of work first
-  const int rem = idx - (idx / per_qt) * per_qt;
-  const int b = rem / nh;
-  it.head = rem - b * nh;
-  it.seq0 = cu_seqlens[b];
-  it.len = cu_seqlens[b + 1] - it.seq0;
-  it.q0 = qt * kTcQ;
-  it.kvh = it.head / (nh / nkv);
-  const int kv_end = min(it.len, it.q0 + kTcQ);       // causal: keys 0 .. kv_end-1
-  it.nt = it.q0 < it.len ? (kv_end + kTcKV - 1) / kTcKV : 0;
-  return it.nt > 0;
-}
-
-// does any lane of the warp want it?  One vote instruction (the shuffle tree the first version used was five dependent shuffles on the
-// softmax warps' critical path: 8 % of the kernel's stall samples); tests/cuda_on_cpu has shuffles only
-__device__ __forceinline__ bool tc_warp_any(bool p) {
-#ifndef CTS_HOST_SHIM
-  return __any_sync(0xffffffffu, p) != 0;
-#else
-  int v = p ? 1 : 0;
-  for (int o = 16; o > 0; o >>= 1) v |= __shfl_xor_sync(0xffffffffu, v, o);
-  return v != 0;
-#endif
-}
-
-// Measured and rejected (profiles/r2_attention_two_warps_per_row_block_rejected.json, git history): two softmax warps per 32-row block,
-// each taking half of a tile's key columns and exchanging the half-row maxima over a 64-thread named barrier -- half the instructions per
-// warp and tile, and 5 % SLOWER (301 vs 286 us at 32 x 576, 891 vs 853 us at 4 x 4096): the softmax instruction stream is not the
-// critical path any more; what remains is the chain of barrier round trips (S ready -> P ready -> P.V done) per 64-key tile.
 template <typename T, bool LSE>
-__global__ void __launch_bounds__(kTcThreads, 2)
-attn_prefill_tc5_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-                        const __grid_constant__ CUtensorMap tm_v, const int* __restrict__ cu_seqlens, int nh, int nkv, int batch, int nqt,
-                        float scale, T* __restrict__ out, float* __restrict__ lse) {
-  constexpr int HD = 128;
-  extern __shared__ uint8_t tc_raw[];
-  __shared__ uint64_t q_bar, q_free, kv_full[kTcStages], kv_empty[kTcStages], s_full[2], s_free[2], p_full, p_free, o_done, o_free;
-  __shared__ uint32_t tmem_slot;
-  const uint32_t raw = smem_u32(tc_raw);
-  uint8_t* smem = tc_raw + (((raw + 1023u) & ~1023u) - raw);
-  uint8_t* q_s = smem;                               // 32 KiB: 2 d-halves x [128 x 128 B]
-  uint8_t* p_s = q_s + 2 * kTcQHalf;                 // 16 KiB: [128 x 128 B] (64 kv columns)
-  uint8_t* ring = p_s + kTcQ * 128;                  // kTcStages x 16 KiB: a K or V tile = 2 d-halves x [64 x 128 B]
-
+__global__ void __launch_bounds__(kWgThreads, 2)
+attn_prefill_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
+                          const __grid_constant__ CUtensorMap tm_v, const int* __restrict__ cu_seqlens, int nh, int nkv, float scale,
+                          T* __restrict__ out, float* __restrict__ lse) {
+  extern __shared__ uint8_t wg_raw[];
+  __shared__ uint64_t q_bar, full_bar[kWgStages], empty_bar[kWgStages];
+  constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
+  const uint32_t raw = smem_u32(wg_raw);
+  uint8_t* smem = wg_raw + (((raw + 1023u) & ~1023u) - raw);
+  uint8_t* q_s = smem;                                   // [2 halves][64 rows x 128 B]
+  uint8_t* kv_s = smem + 2 * kWgHalf;                    // [stage][K half 0 | K half 1 | V half 0 | V half 1]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int total_items = nqt * nh * batch;
+  const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+  const int kvh = head / (nh / nkv);
+
   pdl_trigger();
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_q); tma_prefetch_desc(&tm_k); tma_prefetch_desc(&tm_v);
     mbar_init(&q_bar, 1);
-    mbar_init(&q_free, 1);
-    for (int s = 0; s < kTcStages; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&s_full[s], 1); mbar_init(&s_free[s], 4); }
-    mbar_init(&p_full, 4);
-    mbar_init(&p_free, 1);
-    mbar_init(&o_done, 1);
-    mbar_init(&o_free, 4);
+    for (int s = 0; s < kWgStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<256>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;               // S0: cols 0..63, S1: 64..127, O: 128..255
-  pdl_wait();
+  pdl_wait();                                            // Q / K / V / cu_seqlens come from the predecessors
+  const int seq0 = cu_seqlens[b], len = cu_seqlens[b + 1] - seq0;
+  const int q0 = qt * kWgQ;
+  if (q0 >= len) return;                                 // CTA-uniform; nothing was issued yet
+  const int kv_end = min(len, q0 + kWgQ);                // causal: keys 0 .. q0 + 63
+  const int ntiles = (kv_end + kWgKV - 1) / kWgKV;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
-      uint32_t n = 0;                                   // K / V tiles requested so far (ring slot n % kTcStages), over all items
-      uint32_t k = 0;                                   // live items started by this CTA
-      for (int idx = blockIdx.x; idx < total_items; idx += gridDim.x) {
-        TcItem it;
-        if (!tc_item(idx, nqt, nh, nkv, batch, cu_seqlens, it)) continue;
-        if (k > 0) mbar_wait(&q_free, (k - 1) & 1u);     // every QK^T of the previous item has read the Q tile
-        mbar_expect_tx(&q_bar, (uint32_t)(2 * kTcQHalf));
-        tma_load_2d(q_s, &tm_q, &q_bar, it.head * HD, it.seq0 + it.q0, CTS_L2_EVICT_FIRST);
-        tma_load_2d(q_s + kTcQHalf, &tm_q, &q_bar, it.head * HD + 64, it.seq0 + it.q0, CTS_L2_EVICT_FIRST);
-        auto load_tile = [&](const CUtensorMap* tm, int j) {
-          const uint32_t sl = n % kTcStages;
-          mbar_wait(&kv_empty[sl], ((n / kTcStages) & 1u) ^ 1u);
-          mbar_expect_tx(&kv_full[sl], (uint32_t)(2 * kTcKHalf));
-          uint8_t* dst = ring + (size_t)sl * 2 * kTcKHalf;
-          const int row = it.seq0 + j * kTcKV;
-          tma_load_2d(dst, tm, &kv_full[sl], it.kvh * HD, row, CTS_L2_EVICT_LAST);
-          tma_load_2d(dst + kTcKHalf, tm, &kv_full[sl], it.kvh * HD + 64, row, CTS_L2_EVICT_LAST);
-          ++n;
-        };
-        for (int j = 0; j < it.nt; ++j) {                // K_0, K_1, V_0, K_2, V_1, ..., V_{nt-1}
-          load_tile(&tm_k, j);
-          if (j > 0) load_tile(&tm_v, j - 1);
-        }
-        load_tile(&tm_v, it.nt - 1);
-        ++k;
+      mbar_expect_tx(&q_bar, 2u * kWgHalf);
+      tma_load_2d(q_s, &tm_q, &q_bar, head * 128, seq0 + q0, CTS_L2_EVICT_FIRST);
+      tma_load_2d(q_s + kWgHalf, &tm_q, &q_bar, head * 128 + 64, seq0 + q0, CTS_L2_EVICT_FIRST);
+      for (int j = 0; j < ntiles; ++j) {
+        const int s = j % kWgStages;
+        mbar_wait(&empty_bar[s], ((uint32_t)(j / kWgStages) & 1u) ^ 1u);
+        mbar_expect_tx(&full_bar[s], (uint32_t)kWgStageBytes);
+        uint8_t* st = kv_s + (size_t)s * kWgStageBytes;
+        const int row = seq0 + j * kWgKV;
+        tma_load_2d(st, &tm_k, &full_bar[s], kvh * 128, row, CTS_L2_EVICT_LAST);
+        tma_load_2d(st + kWgHalf, &tm_k, &full_bar[s], kvh * 128 + 64, row, CTS_L2_EVICT_LAST);
+        tma_load_2d(st + 2 * kWgHalf, &tm_v, &full_bar[s], kvh * 128, row, CTS_L2_EVICT_LAST);
+        tma_load_2d(st + 3 * kWgHalf, &tm_v, &full_bar[s], kvh * 128 + 64, row, CTS_L2_EVICT_LAST);
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
-      const uint32_t idesc_qk = umma_idesc_f16(kBf16 ? 1 : 0, kTcKV, 128);
-      const uint32_t idesc_pv = umma_idesc_f16(kBf16 ? 1 : 0, 128, 128) | (1u << 16);   // B (= V) is MN-major
-      const uint32_t q_addr = smem_u32(q_s), p_addr = smem_u32(p_s), ring_addr = smem_u32(ring);
-      uint32_t c = 0;                                     // ring tiles consumed so far (same sequence as the producer's)
-      uint32_t t = 0;                                     // S tiles issued so far, over all items (S buffer t & 1)
-      uint32_t pv = 0;                                    // P.V products issued so far, over all items
-      uint32_t k = 0;                                     // live items started
-      auto take = [&]() {
-        const uint32_t sl = c % kTcStages;
-        mbar_wait(&kv_full[sl], (c / kTcStages) & 1u);
-        ++c;
-        return sl;
-      };
-      auto issue_pv = [&](bool first_of_item) {           // O (+)= P V for the oldest P not yet multiplied
-        mbar_wait(&p_full, pv & 1u);
-        const uint32_t sl = take();
-        const uint32_t v_addr = ring_addr + sl * 2 * kTcKHalf;
-        if (first_of_item && k > 0) mbar_wait(&o_free, (k - 1) & 1u);      // the epilogue warps have read the previous item's O
-        tc_fence_after();
+    return;
+  }
+  if (warp > 4) return;
+
+  // ------------------------------ MMA + softmax warpgroup ------------------------------
+  const float sl2 = scale * 1.4426950408889634f;         // softmax in log2 units
+  const int r0 = q0 + acc_row(0), r1 = r0 + 8;           // this thread's two query rows (sequence positions)
+  float o[64];
 #pragma unroll
-        for (int kk = 0; kk < kTcKV / 16; ++kk) {
-          const uint64_t bdesc = umma_desc_mn_sw128(v_addr + (uint32_t)kk * 16 * 128, 2 * kTcKHalf / 2, 1024);
-          umma_f16(tmem_base + 128, umma_desc_k_sw128(p_addr + (uint32_t)kk * 32), bdesc, idesc_pv, (!first_of_item || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&kv_empty[sl]);
-        umma_commit(&p_free);
-        ++pv;
-      };
-      for (int idx = blockIdx.x; idx < total_items; idx += gridDim.x) {
-        TcItem it;
-        if (!tc_item(idx, nqt, nh, nkv, batch, cu_seqlens, it)) continue;
-        mbar_wait(&q_bar, k & 1u);
-        for (int i = 0; i < it.nt; ++i, ++t) {
-          const uint32_t sb = t & 1u;
-          const uint32_t sl = take();
-          const uint32_t k_addr = ring_addr + sl * 2 * kTcKHalf;
-          if (t >= 2) mbar_wait(&s_free[sb], ((t - 2) >> 1) & 1u);      // softmax warps finished reading S[sb]
-          tc_fence_after();
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint32_t q_addr = smem_u32(q_s);
+  mbar_wait(&q_bar, 0);
+  for (int j = 0; j < ntiles; ++j) {
+    const int s = j % kWgStages;
+    mbar_wait(&full_bar[s], (uint32_t)(j / kWgStages) & 1u);
+    const uint32_t k_addr = smem_u32(kv_s + (size_t)s * kWgStageBytes), v_addr = k_addr + 2 * kWgHalf;
+    float sc[32];
 #pragma unroll
-          for (int kk = 0; kk < HD / 16; ++kk) {
-            const uint32_t qoff = (uint32_t)(kk >> 2) * kTcQHalf + (uint32_t)(kk & 3) * 32;
-            const uint32_t koff = (uint32_t)(kk >> 2) * kTcKHalf + (uint32_t)(kk & 3) * 32;
-            umma_f16(tmem_base + sb * kTcKV, umma_desc_k_sw128(q_addr + qoff), umma_desc_k_sw128(k_addr + koff), idesc_qk,
-                     kk > 0 ? 1u : 0u);
-          }
-          umma_commit(&s_full[sb]);
-          umma_commit(&kv_empty[sl]);
-          if (i + 1 == it.nt) umma_commit(&q_free);        // the Q tile may be replaced once these MMAs have completed
-          if (i > 0) issue_pv(i == 1);                     // P.V of the previous tile, behind this tile's QK^T
-        }
-        issue_pv(it.nt == 1);
-        umma_commit(&o_done);
-        ++k;
-      }
+    for (int i = 0; i < 32; ++i) sc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) wgmma_fence_operand(sc[i]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {                     // head_dim 128 = two 64-wide halves x four k16 steps
+      const uint32_t off = (uint32_t)(kk >> 2) * kWgHalf;
+      wgmma_m64k16<64, kIsBf16>(sc, gmma_desc_k_sw128(q_addr + off) + 2 * (kk & 3), gmma_desc_k_sw128(k_addr + off) + 2 * (kk & 3), kk > 0);
     }
-  } else {
-    // ------------------------------ softmax / epilogue warps (thread = query row) ------------------------------
-    const int q = warp & 3;
-    const int r = q * 32 + lane;                          // row inside the tile == TMEM lane
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-    const float sl2 = scale * 1.4426950408889634f;
-    uint32_t t = 0;                                       // S tiles consumed so far, over all items
-    uint32_t k = 0;                                       // live items started
-    for (int idx = blockIdx.x; idx < total_items; idx += gridDim.x) {
-      TcItem it;
-      if (!tc_item(idx, nqt, nh, nkv, batch, cu_seqlens, it)) continue;
-      const int q0 = it.q0, qi = q0 + r;                  // query index inside the sequence
-      float m_run = -INFINITY, l_run = 0.f;               // m_run: the (lazily refreshed) maximum the exponents are taken against, in log2 units
-      for (int j = 0; j < it.nt; ++j, ++t) {
-        const int kv0 = j * kTcKV;
-        const bool need_mask = kv0 + kTcKV - 1 > q0;      // CTA-uniform: the tile reaches past the first query row
-        const uint32_t sb = t & 1u;
-        const uint32_t s_addr = lane_base + sb * kTcKV;
-        mbar_wait(&s_full[sb], (t >> 1) & 1u);
-        tc_fence_after();
-        uint32_t sv[kTcKV];
+    wgmma_commit();
+    wgmma_wait<0>();
 #pragma unroll
-        for (int c = 0; c < kTcKV; c += 16) tmem_ld_32x32b_x16(s_addr + (uint32_t)c, sv + c);     // all four loads in flight, ONE wait
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_free[sb]);          // S[sb] is in registers: QK^T of tile t+2 may overwrite it
-        // The softmax warps are instruction-issue bound (ncu of the first single-pass version: ~1 500 instructions per warp and tile,
-        // 45 % issue-active, tensor pipe 15 %), so the per-element work is what the arithmetic needs and no more: FMNMX on the raw score,
-        // one FFMA + one MUFU.EX2 + one FADD, half a conversion; the causal select only in the (CTA-uniform) diagonal tiles.
-        float mx = -INFINITY;
-        if (need_mask) {
+    for (int i = 0; i < 32; ++i) wgmma_fence_operand(sc[i]);
+    // causal + length mask, scale, row maxima (a row lives in the 4 lanes of a quad)
+    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-          for (int e = 0; e < kTcKV; ++e) mx = fmaxf(mx, kv0 + e <= qi ? __uint_as_float(sv[e]) : -INFINITY);
-        } else {
+    for (int i = 0; i < 32; ++i) {
+      const int h = (i >> 1) & 1, row = h ? r1 : r0, col = j * kWgKV + acc_col(i);
+      const float v = (col > row || col >= len) ? -INFINITY : sc[i] * sl2;
+      sc[i] = v;
+      mx[h] = fmaxf(mx[h], v);
+    }
+    float corr[2];
 #pragma unroll
-          for (int e = 0; e < kTcKV; ++e) mx = fmaxf(mx, __uint_as_float(sv[e]));
-        }
-        mx *= sl2;                                        // sl2 > 0: scaling commutes with the maximum
-        // lazy maximum: keep the old one unless the tile exceeds it by more than 8 (then P <= 2^8 everywhere)
-        float alpha = 1.f;
-        bool rescale = false;
-        if (mx > m_run + 8.f) {
-          rescale = m_run > -INFINITY;                    // the first finite maximum needs no rescale: l and O are still zero
-          alpha = rescale ? tc_ex2(m_run - mx) : 1.f;
-          m_run = mx;
-        }
-        const float mneg = m_run > -INFINITY ? -m_run : 0.f;
-        l_run *= alpha;
-        uint4 pk[kTcKV / 8];
-        float ls0 = 0.f, ls1 = 0.f;                       // two partial row sums: half the length of the dependent FADD chain
-        if (need_mask) {
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m_run[h], mx[h]);
+      corr[h] = m_new == -INFINITY ? 1.f : exp2f(m_run[h] - m_new);
+      m_run[h] = m_new;
+    }
+    float sum[2] = {0.f, 0.f};
+    uint32_t a[4][4];
 #pragma unroll
-          for (int c = 0; c < kTcKV; c += 8) {
-            float pv[8];
+    for (int i = 0; i < 32; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float p0 = m_run[h] == -INFINITY ? 0.f : exp2f(sc[i] - m_run[h]);
+      const float p1 = m_run[h] == -INFINITY ? 0.f : exp2f(sc[i + 1] - m_run[h]);
+      sum[h] += p0 + p1;
+      a[i >> 3][(i >> 1) & 3] = pack2<T>(p0, p1);       // i = 8 kk + 2 e: register e of the k-step kk fragment
+    }
 #pragma unroll
-            for (int e = 0; e < 8; ++e) pv[e] = kv0 + c + e <= qi ? tc_ex2(fmaf(__uint_as_float(sv[c + e]), sl2, mneg)) : 0.f;
-            ls0 += (pv[0] + pv[1]) + (pv[2] + pv[3]);
-            ls1 += (pv[4] + pv[5]) + (pv[6] + pv[7]);
-            pk[c / 8] = pack8<T>(pv);
-          }
-        } else {
+    for (int h = 0; h < 2; ++h) {
+      sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+      sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+      l_run[h] = l_run[h] * corr[h] + sum[h];
+    }
 #pragma unroll
-          for (int c = 0; c < kTcKV; c += 8) {
-            float pv[8];
+    for (int i = 0; i < 64; ++i) o[i] *= corr[(i >> 1) & 1];
 #pragma unroll
-            for (int e = 0; e < 8; ++e) pv[e] = tc_ex2(fmaf(__uint_as_float(sv[c + e]), sl2, mneg));
-            ls0 += (pv[0] + pv[1]) + (pv[2] + pv[3]);
-            ls1 += (pv[4] + pv[5]) + (pv[6] + pv[7]);
-            pk[c / 8] = pack8<T>(pv);
-          }
-        }
-        l_run += ls0 + ls1;
-        if (t > 0) mbar_wait(&p_free, (t - 1) & 1u);      // the previous P.V (of this item or the one before) has completed: P may be overwritten, O rescaled
-        if (tc_warp_any(rescale)) {                       // warp-collective: rows that keep their maximum multiply by 1
-          tc_fence_after();
-#pragma unroll 1
-          for (int c = 0; c < HD; c += 16) {
-            uint32_t v[16];
-            tmem_ld_32x32b_x16(lane_base + 128u + (uint32_t)c, v);
-            tmem_ld_wait();
+    for (int i = 0; i < 64; ++i) wgmma_fence_operand(o[i]);
+    wgmma_fence();
 #pragma unroll
-            for (int e = 0; e < 16; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * alpha);
-            tmem_st_32x32b_x16(lane_base + 128u + (uint32_t)c, v);
-          }
-          tmem_st_wait();
-          tc_fence_before();
-        }
-        // P[r][0..63] -> K-major swizzled tile (row r, 16-byte chunk ch at ch ^ (r & 7))
+    for (int kk = 0; kk < 4; ++kk)                       // 16 keys per step: V rows kk*16.., both 64-wide halves of head_dim
+      wgmma_m64n128k16_rs_tb<kIsBf16>(o, a[kk], gmma_desc_sw128(v_addr + (uint32_t)kk * 16 * 128, kWgHalf, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
 #pragma unroll
-        for (int ch = 0; ch < kTcKV / 8; ++ch)
-          *reinterpret_cast<uint4*>(p_s + (uint32_t)r * 128 + ((ch ^ (r & 7)) << 4)) = pk[ch];
-        fence_proxy_async_smem();                         // P must be visible to the tensor core (async proxy)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full);
-      }
-      // ---- epilogue: O / l   (tcgen05.ld is warp-collective: every lane loads, rows inside the sequence are stored)
-      mbar_wait(&o_done, k & 1u);
-      tc_fence_after();
-      {
-        const float inv = l_run > 0.f ? 1.0f / l_run : 0.f;
-        const bool row_ok = qi < it.len;
-        T* o_g = out + ((long long)it.seq0 + (row_ok ? qi : 0)) * nh * HD + (long long)it.head * HD;
-#pragma unroll 1
-        for (int c = 0; c < HD; c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x16(lane_base + 128u + (uint32_t)c, v);
-          tmem_ld_32x32b_x16(lane_base + 128u + (uint32_t)c + 16u, v + 16);
-          tmem_ld_wait();
-          if (c + 32 == HD) {                             // O is in registers: the next item's first P.V may overwrite it
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&o_free);
-          }
-          if (row_ok) {
-            float f[32];
+    for (int i = 0; i < 64; ++i) wgmma_fence_operand(o[i]);
+    if (threadIdx.x == 0) mbar_arrive(&empty_bar[s]);   // the warpgroup's MMAs of this stage are complete
+  }
+  // ------------------------------ epilogue: O / l ------------------------------
+  const long long ld = (long long)nh * 128;
 #pragma unroll
-            for (int e = 0; e < 32; ++e) f[e] = __uint_as_float(v[e]) * inv;
+  for (int h = 0; h < 2; ++h) {
+    const int row = h ? r1 : r0;
+    if (row >= len) continue;
+    const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
+    T* orow = out + (long long)(seq0 + row) * ld + head * 128;
 #pragma unroll
-            for (int e = 0; e < 32; e += 8) *reinterpret_cast<uint4*>(o_g + c + e) = pack8<T>(f + e);
-          }
-        }
-        if constexpr (LSE) {
-          if (row_ok) lse[((long long)it.seq0 + qi) * nh + it.head] = l_run > 0.f ? m_run * 0.6931471805599453f + logf(l_run) : -INFINITY;   // m_run is in log2 units
-        }
-      }
-      ++k;
+    for (int i = 2 * h; i < 64; i += 4)                  // registers of row h: i with (i >> 1) & 1 == h, in pairs of columns
+      *reinterpret_cast<uint32_t*>(orow + acc_col(i)) = pack2<T>(o[i] * inv, o[i + 1] * inv);
+    if constexpr (LSE) {
+      if ((lane & 3) == 0)
+        lse[(long long)(seq0 + row) * nh + head] = l_run[h] > 0.f ? m_run[h] * 0.6931471805599453f + logf(l_run[h]) : -INFINITY;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<256>(tmem_base);
 }
 
 // ================================================================================================
@@ -916,35 +727,30 @@ static int attn_prefill_impl(cts_ctx* ctx, const void* q, const void* k, const v
   if (batch == 0 || max_seqlen == 0) return CTS_OK;
   CTS_CHECK_ARG(ctx, batch <= 65535 && nh <= 65535, "grid");
   cudaStream_t st = (cudaStream_t)stream;
-  if (head_dim == 128 && !ctx->force_wmma_attention) {
-    // tcgen05 path: Q/K/V through TMA tensor maps over the packed [tokens, heads*128] activations
+  if (head_dim == 128) {
+    // wgmma path: Q/K/V through TMA tensor maps over the packed [tokens, heads*128] activations
     const long long total_tokens = total_tokens_hint > 0 ? total_tokens_hint : (long long)batch * max_seqlen;
     CUtensorMap tm_q, tm_k, tm_v;
-    int rc = cts_make_tmap_2d(ctx, &tm_q, q, total_tokens, (long long)nh * 128, (long long)nh * 128, kTcQ, dtype == CTS_BF16);
+    int rc = cts_make_tmap_2d(ctx, &tm_q, q, total_tokens, (long long)nh * 128, (long long)nh * 128, kWgQ, dtype == CTS_BF16);
     if (rc) return rc;
-    rc = cts_make_tmap_2d(ctx, &tm_k, k, total_tokens, (long long)nkv * 128, (long long)nkv * 128, kTcKV, dtype == CTS_BF16);
+    rc = cts_make_tmap_2d(ctx, &tm_k, k, total_tokens, (long long)nkv * 128, (long long)nkv * 128, kWgKV, dtype == CTS_BF16);
     if (rc) return rc;
-    rc = cts_make_tmap_2d(ctx, &tm_v, v, total_tokens, (long long)nkv * 128, (long long)nkv * 128, kTcKV, dtype == CTS_BF16);
+    rc = cts_make_tmap_2d(ctx, &tm_v, v, total_tokens, (long long)nkv * 128, (long long)nkv * 128, kWgKV, dtype == CTS_BF16);
     if (rc) return rc;
-    const int nqt = (max_seqlen + kTcQ - 1) / kTcQ;
-    long long items = (long long)nqt * nh * batch;
-    CTS_CHECK_ARG(ctx, items < 2147483647LL, "too many (query tile, head, sequence) items");
-    long long ctas = 2LL * ctx->sm_count;                 // persistent: two CTAs per SM (shared memory and TMEM columns allow exactly two)
-    if (ctas > items) ctas = items;
-    dim3 g5((unsigned)ctas, 1, 1);
-    const size_t smem5 = (size_t)kTcSmem + 1024;
-#define TC5_LAUNCH(TT, LSEV)                                                                                 \
+    dim3 gw((unsigned)((max_seqlen + kWgQ - 1) / kWgQ), (unsigned)nh, (unsigned)batch);
+    const size_t smem_w = (size_t)kWgSmem + 1024;
+#define WG_LAUNCH(TT, LSEV)                                                                                  \
   {                                                                                                          \
-    auto kern = attn_prefill_tc5_kernel<TT, LSEV>;                                                           \
-    CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem5));      \
-    CTS_CUDA(ctx, launch_pdl(kern, g5, dim3(kTcThreads), smem5, st, 1, tm_q, tm_k, tm_v, cu_seqlens, nh, nkv, batch, nqt, scale, (TT*)out, lse)); \
+    auto kern = attn_prefill_wgmma_kernel<TT, LSEV>;                                                         \
+    CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));     \
+    CTS_CUDA(ctx, launch_pdl(kern, gw, dim3(kWgThreads), smem_w, st, 1, tm_q, tm_k, tm_v, cu_seqlens, nh, nkv, scale, (TT*)out, lse)); \
   }
     if (dtype == CTS_BF16) {
-      if (lse) TC5_LAUNCH(__nv_bfloat16, true) else TC5_LAUNCH(__nv_bfloat16, false)
+      if (lse) WG_LAUNCH(__nv_bfloat16, true) else WG_LAUNCH(__nv_bfloat16, false)
     } else {
-      if (lse) TC5_LAUNCH(__half, true) else TC5_LAUNCH(__half, false)
+      if (lse) WG_LAUNCH(__half, true) else WG_LAUNCH(__half, false)
     }
-#undef TC5_LAUNCH
+#undef WG_LAUNCH
     return CTS_OK;
   }
   dim3 grid((unsigned)((max_seqlen + kPfQ - 1) / kPfQ), (unsigned)nh, (unsigned)batch);

@@ -9,9 +9,9 @@
 // query tiles at or below the diagonal; dK/dV of a kv head are summed over its q heads in registers -> no atomics, fixed
 // summation order).  S / dP are recomputed in both kernels (2x QK^T-sized work) in exchange for determinism.
 //
-// Round-1 implementation: HMMA through nvcuda::wmma (m16n16k16, fp32 accumulate), cp.async double buffering -- the same
-// building blocks as the validated round-0 prefill kernel (attention.cu).  The tcgen05/TMEM version is a round-2 item
-// (DESIGN.md); no mbarrier / flag spin anywhere in this file.
+// HMMA through nvcuda::wmma (m16n16k16, fp32 accumulate), cp.async double buffering; no mbarrier / flag spin anywhere in this
+// file.  head_dim 128 runs the wgmma kernels of attention_bwd_wgmma.cu by default; these kernels serve head_dim 64 and are the
+// reference the wgmma kernels are tested against (CTS_ATTN_BWD_WGMMA=0).
 #include <mma.h>
 #include <stdlib.h>
 
@@ -399,15 +399,12 @@ attn_bwd_dkv_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
 
 }  // namespace
 
-// tcgen05 / TMEM version for head_dim 128 (attention_bwd_tc5.cu); opt-in until it has been validated on a B200
-int cts_attn_bwd_tc5_launch(cts_ctx* ctx, const void* q, const void* k, const void* v, const void* dout, const float* lse,
-                            const float* delta, const int* cu_seqlens, int batch, int max_seqlen, long long total_tokens, int nh,
-                            int nkv, float scale, void* dq, void* dk, void* dv, int dtype, cudaStream_t st);
-
-// Default since round 2: the tcgen05 backward (head_dim 128) is validated on a B200 against autograd and the HMMA kernels and makes the
-// ChatTS-8B LoRA step 8 % faster (profiles/r2_bench_lora_variants.txt); CTS_ATTN_BWD_TC5=0 selects the HMMA kernels.
-static bool attn_bwd_use_tc5() {          // read per call (host side, once per launch): tests flip it inside one process
-  const char* e = getenv("CTS_ATTN_BWD_TC5");
+// wgmma version for head_dim 128 (attention_bwd_wgmma.cu), the default; CTS_ATTN_BWD_WGMMA=0 selects the HMMA kernels below
+int cts_attn_bwd_wgmma_launch(cts_ctx* ctx, const void* q, const void* k, const void* v, const void* dout, const float* lse,
+                              const float* delta, const int* cu_seqlens, int batch, int max_seqlen, long long total_tokens, int nh,
+                              int nkv, float scale, void* dq, void* dk, void* dv, int dtype, cudaStream_t st);
+static bool attn_bwd_use_wgmma() {        // read per call (host side, once per launch): tests flip it inside one process
+  const char* e = getenv("CTS_ATTN_BWD_WGMMA");
   return !(e && e[0] == '0');
 }
 
@@ -426,7 +423,7 @@ extern "C" int cts_attn_bwd(cts_ctx* ctx, const void* q, const void* k, const vo
   cudaStream_t st = (cudaStream_t)stream;
   const long long rows = total_tokens * nh;
   const unsigned tiles = (unsigned)((max_seqlen + kBwTile - 1) / kBwTile);
-  if (head_dim == 128 && attn_bwd_use_tc5()) {
+  if (head_dim == 128 && attn_bwd_use_wgmma()) {
     if (dtype == CTS_BF16) {
       CTS_CUDA(ctx, launch_pdl(attn_bwd_delta_kernel<__nv_bfloat16>, dim3((unsigned)cdiv_ll(rows, 8)), dim3(256), 0, st, 1,
                                (const __nv_bfloat16*)out, (const __nv_bfloat16*)dout, delta_ws, rows, 128));
@@ -434,8 +431,8 @@ extern "C" int cts_attn_bwd(cts_ctx* ctx, const void* q, const void* k, const vo
       CTS_CUDA(ctx, launch_pdl(attn_bwd_delta_kernel<__half>, dim3((unsigned)cdiv_ll(rows, 8)), dim3(256), 0, st, 1, (const __half*)out,
                                (const __half*)dout, delta_ws, rows, 128));
     }
-    return cts_attn_bwd_tc5_launch(ctx, q, k, v, dout, lse, delta_ws, cu_seqlens, batch, max_seqlen, total_tokens, nh, nkv, scale, dq, dk,
-                                   dv, dtype, st);
+    return cts_attn_bwd_wgmma_launch(ctx, q, k, v, dout, lse, delta_ws, cu_seqlens, batch, max_seqlen, total_tokens, nh, nkv, scale, dq,
+                                     dk, dv, dtype, st);
   }
 #define BW_LAUNCH(TT, HDV)                                                                                                  \
   {                                                                                                                         \

@@ -43,8 +43,8 @@ extern "C" int cts_ctx_create(int device, cts_ctx** out) {
     free(ctx);
     return CTS_ERR_CUDA;
   }
-  if (prop.major != 10) {
-    fprintf(stderr, "chatts_b200: device %d is sm_%d%d; this library contains sm_100a code only\n", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    fprintf(stderr, "chatts_b200: device %d is sm_%d%d; this library contains sm_90a code only\n", device, prop.major,
             prop.minor);
     free(ctx);
     return CTS_ERR_UNSUPPORTED;
@@ -64,14 +64,12 @@ extern "C" int cts_ctx_create(int device, cts_ctx** out) {
   ctx->encode_tiled = (PFN_cuTensorMapEncodeTiled_v12000)fn;
   const char* e1 = getenv("CTS_L2_PREFETCH_MB");
   ctx->l2_prefetch_mb = e1 ? atoi(e1) : 0;
-  const char* e3 = getenv("CTS_ATTN_WMMA");
-  ctx->force_wmma_attention = e3 ? atoi(e3) : 0;
   const char* e4 = getenv("CTS_NO_PERSISTENT_GEMM");
   ctx->no_persistent_gemm = e4 ? atoi(e4) : 0;
   const char* e5 = getenv("CTS_NORM_CLUSTER");
   ctx->norm_cluster = e5 ? atoi(e5) : 8;
   const char* e2 = getenv("CTS_DECODE_SMEM_KB");
-  ctx->decode_stages = e2 ? atoi(e2) : 75;   // 3 CTAs/SM x 3-4 stages measured best on B200 (profiles/r1_sweep_decode_gemm.txt)
+  ctx->decode_stages = e2 ? atoi(e2) : 75;   // shared-memory ring of a decode GEMM CTA: 3 CTAs per SM of 3-4 stages each
   // a few zero-initialised device words for kernels that synchronise through global counters (the fused TS encoder's grid barrier);
   // allocated here so that nothing is allocated inside a CUDA-graph capture
   {
@@ -91,7 +89,7 @@ extern "C" int cts_ctx_create(int device, cts_ctx** out) {
   const char* e6 = getenv("CTS_NEXT_PREFETCH");
   ctx->no_next_prefetch = (e6 && atoi(e6) == 0) ? 1 : 0;
   const char* e7 = getenv("CTS_NEXT_PREFETCH_MB");
-  ctx->next_prefetch_mb = e7 ? atoi(e7) : 0;     // off by default: measured slower on a B200 (profiles/r2_next_prefetch_ab.txt)
+  ctx->next_prefetch_mb = e7 ? atoi(e7) : 0;     // off by default: the prefetched bytes are read twice (once into L2, once by the GEMM)
   *out = ctx;
   return CTS_OK;
 }

@@ -11,7 +11,7 @@
 //   phase 7  bias + (Qwen3 q/k norm) + RoPE + paged KV write of the next layer
 //
 // (modeling_qwen2.py:269-310 minus the attention itself; the per-phase arithmetic and rounding points are the ones of the
-// stand-alone kernels in gemm_tcgen05.cu / elementwise.cu.)  Why: a decode step was ~440 dependent kernels whose
+// stand-alone kernels in gemm_tcgen05.cu (the wgmma GEMMs) / elementwise.cu.)  Why: a decode step was ~440 dependent kernels whose
 // boundaries cost ~3-4 us each in the captured graph; here the phases are separated by grid barriers (one atomic + an
 // acquire spin, ~1 us) and -- the main point -- the TMA producer keeps streaming: as soon as a CTA has issued the last
 // weight tile of a GEMM phase it pre-loads the first `stages` WEIGHT tiles of the NEXT GEMM phase into the shared-memory
@@ -19,7 +19,7 @@
 // phases run under a full ring.
 //
 // One CTA owns at most one (128-row tile, K-split) unit per GEMM phase (the grid is a single wave: 3 CTAs per SM); warp
-// roles are those of gemm_tn_kernel (warp 0 TMA producer, warp 1 TMEM + tcgen05.mma issuer, warps 2..5 epilogue); the
+// roles are those of gemm_tn_kernel (warps 0..3 the wgmma warpgroup and its epilogue, warp 4 TMA producer); the
 // elementwise phases use all 192 threads of all CTAs.  Every wait is bounded (trap instead of hang).
 #include <cooperative_groups.h>
 
@@ -30,7 +30,7 @@
 
 namespace {
 
-constexpr int kBM = 128, kBK = 64, kUmmaK = 16, kThreads = 192, kMaxStages = 8;
+constexpr int kBM = 128, kBK = 64, kThreads = 192, kMaxStages = 8;
 constexpr int kNormChunks = 8;     // CTAs per token in the RMSNorm phases
 
 struct ChainGemm {
@@ -69,15 +69,12 @@ decode_chain_kernel(const __grid_constant__ CUtensorMap tm_wo, const __grid_cons
                     const __grid_constant__ CUtensorMap tm_ao, const __grid_constant__ CUtensorMap tm_xn,
                     const __grid_constant__ CUtensorMap tm_act, const ChainParams p) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages], acc_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t full_bar[kMaxStages], empty_bar[kMaxStages];
   __shared__ float red_s[kThreads / 32];
 
   constexpr int kABytes = kBM * kBK * 2;
   constexpr int kStage = kABytes + BN * kBK * 2;
-  constexpr int kCols = BN <= 32 ? 32 : 64;
   constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
-  constexpr uint32_t idesc = umma_idesc_f16(kIsBf16 ? 1 : 0, BN, kBM);
 
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -90,20 +87,14 @@ decode_chain_kernel(const __grid_constant__ CUtensorMap tm_wo, const __grid_cons
     tma_prefetch_desc(&tm_wo); tma_prefetch_desc(&tm_wgu); tma_prefetch_desc(&tm_wd); tma_prefetch_desc(&tm_wqkv);
     tma_prefetch_desc(&tm_ao); tma_prefetch_desc(&tm_xn); tma_prefetch_desc(&tm_act);
     for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&acc_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<kCols>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
   // ---- running pipeline state (persists across phases)
   uint32_t it_p = 0;          // K blocks whose A tile the producer has issued (producer lane only)
   uint32_t it_b = 0;          // K blocks whose B tile the producer has issued (<= it_p)
-  uint32_t it_m = 0;          // K blocks consumed by the MMA lane
-  uint32_t acc_uses = 0;      // completed accumulators of this CTA (epilogue + MMA lanes track it identically)
+  uint32_t it_m = 0;          // K blocks consumed by the MMA warpgroup
   int n_bar = 0;              // grid barriers passed
 
   auto grid_barrier = [&]() {
@@ -174,7 +165,7 @@ decode_chain_kernel(const __grid_constant__ CUtensorMap tm_wo, const __grid_cons
     int f0 = 0, kb0 = 0, nkb = 0, split = 0;
     const bool active = unit_of(gi, f0, kb0, nkb, split);
     const ChainGemm& g = p.g[gi];
-    if (warp == 0) {
+    if (warp == 4) {
       if (lane == 0) {
         if (active) {
           int done = 0;
@@ -188,43 +179,29 @@ decode_chain_kernel(const __grid_constant__ CUtensorMap tm_wo, const __grid_cons
         }
         prefetch_next_gemm(next_gi);                 // keep the HBM stream going across the coming barrier(s)
       }
-    } else if (warp == 1) {
-      if (lane == 0 && active) {
-        for (int i = 0; i < nkb; ++i, ++it_m) {
-          const int s = it_m % stages;
-          mbar_wait(&full_bar[s], (it_m / stages) & 1u);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
-          const uint64_t a_desc = umma_desc_k_sw128(a_addr), b_desc = umma_desc_k_sw128(a_addr + kABytes);
-#pragma unroll
-          for (int kk = 0; kk < kBK / kUmmaK; ++kk) {
-            const uint64_t adv = (uint64_t)(kk * ((kUmmaK * 2) >> 4));
-            umma_f16(tmem_base, a_desc + adv, b_desc + adv, idesc, (i > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&acc_bar);
+    } else if (warp < 4 && active) {
+      Acc128<BN> acc;
+      acc.zero();
+      for (int i = 0; i < nkb; ++i, ++it_m) {
+        const int s = it_m % stages;
+        mbar_wait(&full_bar[s], (it_m / stages) & 1u);
+        const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
+        acc.template mma_kblock<kIsBf16>(a_addr, a_addr + kABytes, i == 0);
+        wgmma_wait<1>();
+        if (i > 0 && tid == 0) mbar_arrive(&empty_bar[(it_m - 1) % stages]);
       }
-    } else if (active) {
-      mbar_wait(&acc_bar, acc_uses & 1u);
-      tc_fence_after();
-      const int q = warp & 3;
-      const long long f = (long long)f0 + q * 32 + lane;
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
+      wgmma_wait<0>();
+      if (nkb > 0 && tid == 0) mbar_arrive(&empty_bar[(it_m - 1) % stages]);
       float* dst = p.ws + (long long)split * T_ * g.n;
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 16) {
-        if (c >= T_) break;
-        uint32_t v[16];
-        tmem_ld_32x32b_x16(lane_addr + (uint32_t)c, v);
-        tmem_ld_wait();
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (c + j < T_ && f < g.n) dst[(long long)(c + j) * g.n + f] = __uint_as_float(v[j]);
-      }
-      tc_fence_before();
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) {
+          const long long f = (long long)f0 + 64 * h + acc_row(i);
+          const int c = acc_col(i);
+          if (c < T_ && f < g.n) dst[(long long)c * g.n + f] = acc.d[h][i];
+        }
     }
-    if (active) ++acc_uses;
   };
 
   // ------------------------------------------------------------------ residual + RMSNorm (two sub-phases, 8 CTAs per token)
@@ -400,7 +377,7 @@ decode_chain_kernel(const __grid_constant__ CUtensorMap tm_wo, const __grid_cons
       if ((ph & 1) == 0) return ph >> 1;
     return -1;
   };
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     // weights of the first GEMM phase of this launch: in flight before anything else
     const int first = (pb & 1) == 0 ? (pb >> 1) : next_gemm_after(pb);
     prefetch_next_gemm(first);
@@ -420,9 +397,7 @@ decode_chain_kernel(const __grid_constant__ CUtensorMap tm_wo, const __grid_cons
   }
 
   // ---- teardown: the last CTA to leave resets the barrier counters for the next launch
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<kCols>(tmem_base);
   if (tid == 0) {
     __threadfence();
     const int done = atomicAdd(&p.sync[1], 1) + 1;

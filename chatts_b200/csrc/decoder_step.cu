@@ -107,7 +107,7 @@ extern "C" int cts_decoder_step(cts_ctx* ctx, const cts_decoder_step_args* a, vo
 }
 
 // cts_ts_encode: A3..A7 of the TS encoder from one C call (chatts_vllm.py:93-193 + the row scatter of :569-573): patch counts ->
-// patchify -> num_layers x [tcgen05 GEMM (+ split-K tail) with bias / exact-erf GELU], the last layer scattering its rows
+// patchify -> num_layers x [wgmma GEMM (+ split-K tail) with bias / exact-erf GELU], the last layer scattering its rows
 // through row_map into the embedding sequence.  `total_rows` (= sum of patch counts) is a HOST number: the caller sizes the
 // merged sequence with it anyway (it comes from its own mask arithmetic or from a copy of cts_ts_patch_count's output).
 // Same launches as chatts_b200/ts_encoder.py:TimeSeriesEmbedding.encode.

@@ -167,8 +167,7 @@ reduce_residual_rmsnorm_kernel(const float* __restrict__ part, int S, const T* _
 
 // Plain RMSNorm of many rows (prefill-sized T, no partials to reduce: the GEMM before it applied the residual in its epilogue): ONE WARP
 // per row, the row held in registers as packed 16-byte vectors between the two passes, warp shuffles only -- no block barrier.  The
-// one-CTA-per-token kernel above spends two __syncthreads and a shared-memory round trip per 10 KB row: 0.21 ms per launch at 18 432 x
-// 5 120 (1.8 TB/s; profiles/r2_prefill_summary.txt), 5 % of the prefill.
+// one-CTA-per-token kernel above spends two __syncthreads and a shared-memory round trip per 10 KB row.
 constexpr int kRowWarps = 8;
 
 template <typename T, int NVW>

@@ -1,9 +1,8 @@
 // chatts_b200 -- decode GEMM with the split-K reduction AND the projection's tail fused in, through a thread-block cluster.
 //
-// The decode step is nine dependent stages per layer (DESIGN.md section 6: 84 us of weight stream + 19 us of attention +
-// ~35 us of small kernels and ramps).  Four of the nine exist only because the skinny decode GEMMs split K over CTAs and a
+// The decode step is nine dependent stages per layer (weight stream, attention, small kernels and their ramps).  Four of the nine exist only because the skinny decode GEMMs split K over CTAs and a
 // second kernel has to add the fp32 partials before it can apply bias / RoPE / SwiGLU / the residual.  Here the K splits of
-// one 128-feature tile form ONE CLUSTER (grid.z = split <= 8 = cluster.z): every CTA runs the same TMA -> tcgen05 -> TMEM
+// one 128-feature tile form ONE CLUSTER (grid.z = split <= 8 = cluster.z): every CTA runs the same TMA -> wgmma -> registers
 // mainloop as gemm_tn_kernel, parks its fp32 accumulator tile in its own shared memory, and after a cluster barrier the
 // CTAs reduce disjoint TOKENS of the tile over distributed shared memory (split order: the same summation order as the
 // stand-alone reduce kernels, so results are bit-identical to the multi-kernel path) and apply the tail in place:
@@ -38,7 +37,7 @@ namespace {
 
 namespace cg = cooperative_groups;
 
-constexpr int kBM = 128, kBK = 64, kUmmaK = 16, kThreads = 192, kMaxStages = 12;
+constexpr int kBM = 128, kBK = 64, kThreads = 192, kMaxStages = 12;
 
 struct FusedParams {
   long long n, k, t;
@@ -119,15 +118,12 @@ gemm_decode_fused_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_
   CTS_DYN_SMEM(smem_raw);
   __shared__ uint64_t full_bar[kMaxStages];
   __shared__ uint64_t empty_bar[kMaxStages];
-  __shared__ uint64_t acc_bar;
-  __shared__ uint32_t tmem_slot;
   __shared__ float xch[kBM];            // tile-local exchange (SwiGLU up values / RoPE partners)
   __shared__ float red[4];              // per-warp partial sums of the q/k RMSNorm statistic
   __shared__ float rstd_s[32];          // NORM_IN: rsqrt(mean(h^2) + eps) of every token
 
   constexpr int kABytes = kBM * kBK * 2;
   constexpr int kStage = kABytes + BN * kBK * 2;
-  constexpr int kCols = 32;
   constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
   static_assert(BN <= 32, "decode-sized token tile");
 
@@ -150,18 +146,13 @@ gemm_decode_fused_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_w);
     tma_prefetch_desc(&tm_x);
-    // NORM_IN: a stage is full when the weight tile has landed (TMA, expect_tx) AND the four epilogue warps have written B
-    for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], NORM_IN ? 5 : 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&acc_bar, 1);
+    // NORM_IN: the full barrier covers the weight tile only; the MMA warpgroup writes B itself right before its MMAs
+    for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<kCols>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------ TMA producer (as gemm_tn_kernel: weights before the dependency wait) ------------------------------
     if (lane == 0) {
       const int npre = nkb < stages ? nkb : stages;
@@ -186,32 +177,14 @@ gemm_decode_fused_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_
       }
       CTS_TRACE(CTS_TK_FUSED, 2);
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(kIsBf16 ? 1 : 0, BN, kBM);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % stages;
-        mbar_wait(&full_bar[s], ((uint32_t)(i / stages)) & 1u);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
-        const uint64_t a_desc = umma_desc_k_sw128(a_addr), b_desc = umma_desc_k_sw128(a_addr + kABytes);
-#pragma unroll
-        for (int kk = 0; kk < kBK / kUmmaK; ++kk) {
-          const uint64_t adv = (uint64_t)(kk * ((kUmmaK * 2) >> 4));
-          umma_f16(tmem_base, a_desc + adv, b_desc + adv, idesc, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(&acc_bar);
-    }
-  } else {
+  } else if (warp < 4) {
+    // ------------------------------ MMA warpgroup ------------------------------
     pdl_wait();
+    const int et = (int)threadIdx.x;                          // 0..127
     if (NORM_IN) {
-      // ------------------------------ B-operand producers: xn = norm_w * dtype(h * rstd) written as the swizzled K-major token tile ------------------------------
+      // B operand: xn = norm_w * dtype(h * rstd) written as the swizzled K-major token tile of each stage
       // (modeling_qwen2.py:258-263 -- the same values the stand-alone RMSNorm kernel stores, without the launch and the round trip;
       //  the row statistic comes from the per-tile sums of squares the previous fused RESIDUAL projection left in ssq_in)
-      const int et = (int)threadIdx.x - 64;                   // 0..127 inside the epilogue group
       if (et < BN) {
         float tot = 0.f;
         if (et < T_)
@@ -219,17 +192,20 @@ gemm_decode_fused_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_
         rstd_s[et] = 1.0f / sqrtf(tot / (float)p.k + p.norm_eps);
       }
       named_bar_sync(1, 128);
-      const T* hsrc = reinterpret_cast<const T*>(p.norm_h);
-      const T* nw = reinterpret_cast<const T*>(p.norm_w);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % stages;
-        mbar_wait(&empty_bar[s], (((uint32_t)(i / stages)) & 1u) ^ 1u);       // the MMAs that read this slot have completed
-        uint8_t* bt = smem + (size_t)s * kStage + kABytes;                      // [BN rows x 128 B], 128B swizzle
+    }
+    const T* hsrc = reinterpret_cast<const T*>(p.norm_h);
+    const T* nw = reinterpret_cast<const T*>(p.norm_w);
+    Acc128<BN> acc;
+    acc.zero();
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % stages;
+      if (NORM_IN) {                                          // slot s was last read by the MMAs of block i - stages: complete
+        uint8_t* bt = smem + (size_t)s * kStage + kABytes;    // [BN rows x 128 B], 128B swizzle
         for (int it = et; it < BN * 8; it += 128) {
           const int t = it >> 3, ch = it & 7;
           const long long k0 = (long long)(kb0 + i) * kBK + ch * 8;
           uint4 o = make_uint4(0u, 0u, 0u, 0u);
-          if (t < T_ && k0 < p.k) {                                             // k is a multiple of 8 (16-byte rows)
+          if (t < T_ && k0 < p.k) {                           // k is a multiple of 8 (16-byte rows)
             float hv[8], wv[8], xv[8];
             unpack8<T>(*reinterpret_cast<const uint4*>(hsrc + (long long)t * p.k + k0), hv);
             unpack8<T>(*reinterpret_cast<const uint4*>(nw + k0), wv);
@@ -240,34 +216,23 @@ gemm_decode_fused_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_
           }
           *reinterpret_cast<uint4*>(bt + (uint32_t)t * 128 + ((ch ^ (t & 7)) << 4)) = o;
         }
-        fence_proxy_async_smem();                                               // generic-proxy writes -> visible to the tensor core
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&full_bar[s]);
+        fence_proxy_async_smem();                             // generic-proxy writes -> visible to the tensor core
+        named_bar_sync(1, 128);
       }
+      mbar_wait(&full_bar[s], ((uint32_t)(i / stages)) & 1u);
+      const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
+      acc.template mma_kblock<kIsBf16>(a_addr, a_addr + kABytes, i == 0);
+      wgmma_wait<1>();
+      if (i > 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[(i - 1) % stages]);
     }
+    wgmma_wait<0>();
+    if (nkb > 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[(nkb - 1) % stages]);
     // ------------------------------ epilogue, part A: park this split's fp32 tile in shared memory ------------------------------
-    if (nkb > 0) {
-      mbar_wait(&acc_bar, 0);
-      tc_fence_after();
-    }
-    const int q = warp & 3;
-    const int ft = q * 32 + lane;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 16) {
-      if (c >= T_) break;                                    // warp-uniform
-      uint32_t v[16];
-      if (nkb > 0) {
-        tmem_ld_32x32b_x16(lane_addr + (uint32_t)c, v);
-        tmem_ld_wait();
-      } else {
+    named_bar_sync(1, 128);                                   // every warp's MMAs are done with the ring
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0u;
-      }
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int j = 0; j < 16; ++j) part_s[(c + j) * kBM + ft] = __uint_as_float(v[j]);
-    }
-    tc_fence_before();
+      for (int i = 0; i < BN / 2; ++i) part_s[acc_col(i) * kBM + 64 * h + acc_row(i)] = acc.d[h][i];
   }
   __syncthreads();
   cluster.sync();                                            // every split's tile is in its CTA's shared memory
@@ -471,9 +436,7 @@ gemm_decode_fused_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_
     }
   }
   cluster.sync();                                            // nobody leaves while a peer still reads its tile
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<kCols>(tmem_base);
   if (threadIdx.x == 0) CTS_TRACE(CTS_TK_FUSED, 3);
   if (p.peer_region != nullptr && threadIdx.x == 0) {        // the last CTA of the grid to finish publishes the next epoch
     __threadfence();

@@ -1,19 +1,21 @@
-// chatts_b200 -- weight-streaming tcgen05 GEMM:  Y[T,N] = X[T,K] * W[N,K]^T  (+ fused epilogues)
+// chatts_b200 -- weight-streaming wgmma GEMM:  Y[T,N] = X[T,K] * W[N,K]^T  (+ fused epilogues)
 //
 // Replaces every nn.Linear on the ChatTS hot path: the TS-encoder MLP (chatts/vllm/chatts_vllm.py:83-91,188)
 // and the Qwen2 projections / lm_head the reference reaches through transformers / vLLM
 // (modeling_qwen2.py:44-48,217-219,245; chatts_vllm.py:595-610).
 //
-// B200-first design ("swap-AB"): the WEIGHT tile is the 128-row MMA operand A (K-major, streamed once from
-// HBM by TMA with an evict-first hint), the TOKENS are the MMA N dimension (operand B, K-major, L2 resident,
-// evict-last).  A decode batch of 1..32 tokens therefore still issues full M=128 tcgen05.mma instructions
-// and the kernel is bound by the HBM stream of W; a prefill of thousands of tokens uses N=256 tiles of the
-// same kernel.  Accumulators live in TMEM (lane = output feature, column = token); the epilogue warps read
-// them with tcgen05.ld and fuse bias / GELU / SwiGLU / residual / split-K partial stores / row scatter.
+// "Swap-AB" design: the WEIGHT tile is the 128-row MMA operand A (K-major, streamed once from HBM by TMA with
+// an evict-first hint), the TOKENS are the MMA N dimension (operand B, K-major, L2 resident, evict-last).  A
+// decode batch of 1..32 tokens therefore still fills the M = 2 x 64 rows of the wgmma instructions and the
+// kernel is bound by the HBM stream of W; longer prompts use N = 64 / 128 tiles of the same kernel.  The
+// accumulator lives in the registers of the MMA warpgroup, which parks it in shared memory (row = output
+// feature, column = token) for the thread-per-feature epilogue: bias / GELU / SwiGLU / residual / split-K
+// partial stores / row scatter.
 //
-//   warp 0      : TMA producer (one elected lane), mbarrier full/empty ring of `stages` slots
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer, tcgen05.commit frees slots
-//   warps 2..5  : epilogue, warp w owns TMEM lanes 32*(w%4) .. +31
+//   warps 0..3  : MMA warpgroup (wgmma.mma_async, both 64-row halves of the tile), then the epilogue;
+//                 warp w owns output features 32*w .. +31 in the epilogue
+//   warp 4      : TMA producer (one elected lane), mbarrier full/empty ring of `stages` slots
+//   warp 5      : idle
 //
 // grid = (ceil(N/128), ceil(T/BN), split_k).
 #include <type_traits>
@@ -24,9 +26,8 @@
 
 namespace {
 
-constexpr int kBM = 128;        // weight rows per tile == UMMA M
+constexpr int kBM = 128;        // weight rows per tile == two wgmma M = 64 halves
 constexpr int kBK = 64;         // K elements per stage == 128 bytes == one 128B-swizzle atom
-constexpr int kUmmaK = 16;      // K per tcgen05.mma for 16-bit inputs
 constexpr int kMaxStages = 12;
 constexpr int kThreads = 192;
 
@@ -43,17 +44,16 @@ struct GemmParams {
   float* splitk_ws;  // CTS_EPI_SPLITK_F32: fp32 [split_k, t, n] scratch
   int* tile_cnt;     // CTS_EPI_SPLITK_F32: arrival counter per output tile (zero-initialised, self-resetting)
   int l2_prefetch;   // K blocks of W this CTA prefetches into L2 beyond the shared-memory ring while it waits (decode)
-  int staged;        // 1: epilogue goes TMEM -> registers -> shared-memory tile -> TMA store (big tiles)
+  int staged;        // 1: epilogue goes accumulator -> shared-memory output tile -> TMA store (big tiles)
   // next-GEMM weight prefetch (cts_gemm_args.next_*): units of the next launch = next_tiles x next_split, each reads K blocks
   // [kb_total' * z / split', ...) of the 128-row tile x; this grid prefetches the first next_pf blocks of every unit into L2
   int next_tiles, next_split, next_kb_total, next_pf;
 };
 
 template <int BN, bool DUAL> __host__ __device__ constexpr int stage_bytes() { return kBM * kBK * 2 * (DUAL ? 2 : 1) + BN * kBK * 2; }
-template <int BN, bool DUAL> __host__ __device__ constexpr int tmem_cols() {
-  int c = BN * (DUAL ? 2 : 1);
-  return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512;
-}
+// where the parked fp32 accumulator lives: decode tiles (never staged) reuse the idle pipeline ring, bigger tiles sit behind
+// it because the staged epilogue builds its output / residual tiles in the ring
+template <int BN> __host__ __device__ constexpr bool acc_in_ring() { return BN <= 32; }
 
 template <typename T, int BN, bool DUAL>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -63,14 +63,12 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t full_bar[kMaxStages];
   __shared__ uint64_t empty_bar[kMaxStages];
-  __shared__ uint64_t acc_bar;
   __shared__ uint64_t res_bar;
-  __shared__ uint32_t tmem_slot;
   __shared__ int last_flag;
 
   constexpr int kStage = stage_bytes<BN, DUAL>();
   constexpr int kABytes = kBM * kBK * 2;
-  constexpr int kCols = tmem_cols<BN, DUAL>();
+  constexpr int kLd = acc_ld<BN>();
   constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
 
   // 128B-swizzled tiles need a 1024-byte aligned base
@@ -98,17 +96,12 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 1);
     }
-    mbar_init(&acc_bar, 1);
     mbar_init(&res_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<kCols>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
       // Phase 1 (before the dependency wait): the WEIGHT tiles of the first `stages` K blocks.  Nobody writes
@@ -164,40 +157,34 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(kIsBf16 ? 1 : 0, BN, kBM);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % stages;
-        const uint32_t ph = (uint32_t)(i / stages) & 1u;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
-        const uint64_t a_desc = umma_desc_k_sw128(a_addr);
-        const uint64_t a2_desc = umma_desc_k_sw128(a_addr + kABytes);
-        const uint64_t b_desc = umma_desc_k_sw128(a_addr + kABytes * (DUAL ? 2 : 1));
-#pragma unroll
-        for (int kk = 0; kk < kBK / kUmmaK; ++kk) {
-          // advance 16 elements = 32 bytes inside the swizzle atom: +2 in the (addr >> 4) field
-          const uint64_t adv = (uint64_t)(kk * ((kUmmaK * 2) >> 4));
-          const uint32_t acc = (i > 0 || kk > 0) ? 1u : 0u;
-          umma_f16(tmem_base, a_desc + adv, b_desc + adv, idesc, acc);
-          if (DUAL) umma_f16(tmem_base + BN, a2_desc + adv, b_desc + adv, idesc, acc);
-        }
-        umma_commit(&empty_bar[s]);   // slot reusable once these MMAs have read it
-      }
-      umma_commit(&acc_bar);          // accumulator complete
+  } else if (warp < 4) {
+    // ------------------------------ MMA warpgroup ------------------------------
+    Acc128<BN> acc, acc2;                 // acc2: the w2 (up) product of CTS_EPI_SWIGLU
+    acc.zero();
+    if (DUAL) acc2.zero();
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % stages;
+      mbar_wait(&full_bar[s], (uint32_t)(i / stages) & 1u);
+      const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
+      const uint32_t b_addr = a_addr + kABytes * (DUAL ? 2 : 1);
+      acc.template mma_kblock<kIsBf16>(a_addr, b_addr, i == 0);
+      if (DUAL) acc2.template mma_kblock<kIsBf16>(a_addr + kABytes, b_addr, i == 0);
+      wgmma_wait<DUAL ? 2 : 1>();         // the previous K block's MMAs have read their slot
+      if (i > 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[(i - 1) % stages]);
     }
-  } else {
+    wgmma_wait<0>();
+    if (nkb > 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[(nkb - 1) % stages]);
     // ------------------------------ epilogue ------------------------------
+    named_bar_sync(1, 128);               // every warp's MMAs are done with the ring
+    float* acc_s = reinterpret_cast<float*>(acc_in_ring<BN>() ? smem : smem + (size_t)stages * kStage);
+    acc.store(acc_s, kLd);
+    if (DUAL) acc2.store(acc_s + kBM * kLd, kLd);
     pdl_wait();   // residual / row_map / the output buffers belong to predecessors until now
-    mbar_wait(&acc_bar, 0);
-    tc_fence_after();
+    named_bar_sync(1, 128);
     const int q = warp & 3;
     const long long f = (long long)f0 + q * 32 + lane;
     const bool f_ok = f < p.n;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
+    const int row = q * 32 + lane;
     float bias = 0.f;
     if (p.bias != nullptr && f_ok) bias = DT<T>::to_f(reinterpret_cast<const T*>(p.bias)[f]);
     const int epi = p.epilogue;
@@ -219,9 +206,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       for (int c = 0; c < BN; c += 16) {
         if ((long long)t0 + c >= p.t) break;
         uint32_t v[16], v2[16];
-        tmem_ld_32x32b_x16(lane_addr + (uint32_t)c, v);
-        if (DUAL) tmem_ld_32x32b_x16(lane_addr + (uint32_t)(BN + c), v2);
-        tmem_ld_wait();
+        acc_ld16(acc_s, kLd, row, c, v);
+        if (DUAL) acc_ld16(acc_s + kBM * kLd, kLd, row, c, v2);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const float acc = __uint_as_float(v[j]);
@@ -252,8 +238,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       for (int c = 0; c < BN; c += 16) {
         if ((long long)t0 + c >= p.t) break;
         uint32_t v[16];
-        tmem_ld_32x32b_x16(lane_addr + (uint32_t)c, v);
-        tmem_ld_wait();
+        acc_ld16(acc_s, kLd, row, c, v);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const long long t = (long long)t0 + c + j;
@@ -287,13 +272,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     for (int c = 0; c < BN; c += 16) {
       if ((long long)t0 + c >= p.t) break;   // warp-uniform
       uint32_t v[16], v2[16];
-      tmem_ld_32x32b_x16(lane_addr + (uint32_t)c, v);
-      if (DUAL) tmem_ld_32x32b_x16(lane_addr + (uint32_t)(BN + c), v2);
-      tmem_ld_wait();
-      if (nkb == 0) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { v[j] = 0u; v2[j] = 0u; }
-      }
+      acc_ld16(acc_s, kLd, row, c, v);
+      if (DUAL) acc_ld16(acc_s + kBM * kLd, kLd, row, c, v2);
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const long long t = (long long)t0 + c + j;
@@ -327,25 +307,21 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<kCols>(tmem_base);
   if (threadIdx.x == 0) CTS_TRACE(CTS_TK_GEMM, 3);
 }
 
 // =================================================================================================================
-// Persistent variant for big token counts (prefill): one CTA per SM walks the output tiles (128 features x 256 tokens),
-// the TMA/MMA ring runs continuously across tiles and the accumulator is DOUBLE-BUFFERED in TMEM (2 x 256 columns), so
-// the epilogue of tile i (TMEM -> registers -> shared -> TMA store, residual tile by TMA load) overlaps the mainloop of
-// tile i+1.  Epilogues: NONE / GELU / RESIDUAL, and SWIGLU_IL for gate_up weights stored INTERLEAVED (each 128-row weight
-// tile = 64 gate rows then the 64 matching up rows), which makes SwiGLU tile-local: the "up" warps hand their values to
-// the "gate" warps through shared memory and the tile emits 64 output features.
+// Persistent variant for big token counts (prefill): one CTA per SM walks the output tiles (128 features x 128 tokens) and
+// the TMA ring runs continuously across tiles, so the weight / token loads of tile i+1 stream while the MMA warpgroup runs
+// the epilogue of tile i (accumulator registers -> shared-memory output tile -> TMA store, residual tile by TMA load).
+// Epilogues: NONE / GELU / RESIDUAL, and SWIGLU_IL for gate_up weights stored INTERLEAVED (each 128-row weight tile = 64 gate
+// rows then the 64 matching up rows): gate row r and up row r + 64 sit in the same register of the two accumulator halves, so
+// SwiGLU is thread-local and the tile emits 64 output features.
 // =================================================================================================================
-constexpr int kPBN = 256;
-constexpr int kPStages = 3;
-constexpr int kPStageBytes = kBM * kBK * 2 + kPBN * kBK * 2;     // 48 KiB
-constexpr int kPChunk = 128;                                      // tokens per epilogue chunk
-constexpr int kPOutBytes = kPChunk * kBM * 2;                     // 32 KiB staging tile
+constexpr int kPBN = 128;
+constexpr int kPStages = 4;
+constexpr int kPStageBytes = kBM * kBK * 2 + kPBN * kBK * 2;     // 32 KiB
+constexpr int kPOutBytes = kPBN * kBM * 2;                        // 32 KiB staging tile
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -353,8 +329,7 @@ gemm_tn_persistent_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid
                           const __grid_constant__ CUtensorMap tm_out, const __grid_constant__ CUtensorMap tm_res,
                           const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t full_bar[kPStages], empty_bar[kPStages], tmem_full[2], tmem_empty[2], res_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t full_bar[kPStages], empty_bar[kPStages], res_bar;
   constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -367,9 +342,9 @@ gemm_tn_persistent_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid
   const int nkb = p.kb_total;
   const int epi = p.epilogue;
   // L2-aware rasterisation: the feature tiles are walked in groups of `gm` whose weights (gm x 128 x K) fit in L2; inside
-  // a group the token tiles advance slowly and the gm feature tiles fast, so the ~148 tiles in flight share a few token
-  // tiles and the group's weights stay L2-resident across all token tiles.  DRAM then sees the weights once and the
-  // activations once per group (instead of the weights once per token tile: 20 GB per gate_up launch before).
+  // a group the token tiles advance slowly and the gm feature tiles fast, so the tiles in flight share a few token tiles
+  // and the group's weights stay L2-resident across all token tiles.  DRAM then sees the weights once and the
+  // activations once per group (instead of the weights once per token tile).
   const int gm = p.l2_prefetch > 0 ? p.l2_prefetch : tiles_m;
   auto tile_coords = [&](int id, int& m_blk, int& n_blk) {
     const int per_group = gm * tiles_n;
@@ -383,17 +358,12 @@ gemm_tn_persistent_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_w); tma_prefetch_desc(&tm_x); tma_prefetch_desc(&tm_out);
     for (int s = 0; s < kPStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 4); }
     mbar_init(&res_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<512>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
       pdl_wait();
@@ -412,115 +382,76 @@ gemm_tn_persistent_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(kIsBf16 ? 1 : 0, kPBN, kBM);
-      uint32_t it = 0, lt = 0;                           // K-block counter, local tile counter
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-        const uint32_t buf = lt & 1u;
-        mbar_wait(&tmem_empty[buf], ((lt >> 1) & 1u) ^ 1u);       // epilogue has drained this accumulator
-        tc_fence_after();
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = it % kPStages;
-          mbar_wait(&full_bar[s], (it / kPStages) & 1u);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + (size_t)s * kPStageBytes);
-          const uint64_t a_desc = umma_desc_k_sw128(a_addr), b_desc = umma_desc_k_sw128(a_addr + kBM * kBK * 2);
-#pragma unroll
-          for (int kk = 0; kk < kBK / kUmmaK; ++kk) {
-            const uint64_t adv = (uint64_t)(kk * ((kUmmaK * 2) >> 4));
-            umma_f16(tmem_base + buf * kPBN, a_desc + adv, b_desc + adv, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tmem_full[buf]);
-      }
-    }
-  } else {
-    // ------------------------------ epilogue warps ------------------------------
+  } else if (warp < 4) {
+    // ------------------------------ MMA warpgroup + epilogue ------------------------------
     pdl_wait();
-    const int q = warp & 3;
-    const int ft = q * 32 + lane;                         // row of the weight tile == TMEM lane
-    uint32_t lt = 0, res_uses = 0;
+    uint32_t it = 0, res_uses = 0;
     T* outp = reinterpret_cast<T*>(out_s);
-    T* resp = reinterpret_cast<T*>(res_s);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
+    const T* resp = reinterpret_cast<const T*>(res_s);
+    const T* biasp = reinterpret_cast<const T*>(p.bias);
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int mb, nb;
       tile_coords(tile, mb, nb);
       const int f0 = mb * kBM, t0 = nb * kPBN;
-      const uint32_t buf = lt & 1u;
-      const long long f = (long long)f0 + ft;
-      float bias = 0.f;
-      if (p.bias != nullptr && f < p.n) bias = DT<T>::to_f(reinterpret_cast<const T*>(p.bias)[f]);
-      mbar_wait(&tmem_full[buf], (lt >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t lane_addr = tmem_base + buf * kPBN + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-      for (int ch = 0; ch < kPBN / kPChunk; ++ch) {
-        const int tc0 = t0 + ch * kPChunk;
-        const bool chunk_live = tc0 < p.t;                // CTA-uniform
-        if (epi == CTS_EPI_RESIDUAL && chunk_live) {
-          if (threadIdx.x == 64) {
-            mbar_expect_tx(&res_bar, (uint32_t)kPOutBytes);
-            tma_load_2d_nohint(res_s, &tm_res, &res_bar, f0, tc0);
-          }
-          mbar_wait(&res_bar, res_uses & 1u);
-          ++res_uses;
-        }
-#pragma unroll 1
-        for (int c = 0; c < kPChunk; c += 16) {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(lane_addr + (uint32_t)(ch * kPChunk + c), v);
-          tmem_ld_wait();
-          if (!chunk_live) continue;
-          if (epi == CTS_EPI_SWIGLU_IL) {
-            if (ft >= 64) {                               // "up" rows: publish dtype(u) for the gate warps
+      if (epi == CTS_EPI_RESIDUAL && threadIdx.x == 0) {  // the residual tile lands while the mainloop runs
+        fence_proxy_async_smem();                         // the previous tile's generic-proxy reads of res_s (ordered by the named barrier) before the TMA write
+        mbar_expect_tx(&res_bar, (uint32_t)kPOutBytes);
+        tma_load_2d_nohint(res_s, &tm_res, &res_bar, f0, t0);
+      }
+      Acc128<kPBN> acc;
+      acc.zero();
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = it % kPStages;
+        mbar_wait(&full_bar[s], (it / kPStages) & 1u);
+        const uint32_t a_addr = smem_u32(smem + (size_t)s * kPStageBytes);
+        acc.template mma_kblock<kIsBf16>(a_addr, a_addr + kBM * kBK * 2, kb == 0);
+        wgmma_wait<1>();
+        if (kb > 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[(it - 1) % kPStages]);
+      }
+      wgmma_wait<0>();
+      if (nkb > 0 && threadIdx.x == 0) mbar_arrive(&empty_bar[(it - 1) % kPStages]);
+      if (epi == CTS_EPI_RESIDUAL) {
+        mbar_wait(&res_bar, res_uses & 1u);
+        ++res_uses;
+      }
+      if (epi == CTS_EPI_SWIGLU_IL) {
 #pragma unroll
-              for (int j = 0; j < 16; ++j) resp[(c + j) * 64 + (ft - 64)] = DT<T>::from_f(__uint_as_float(v[j]));
-            }
-            named_bar_sync(2, 128);
-            if (ft < 64) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const float g = rnd<T>(__uint_as_float(v[j]));
-                const float u = DT<T>::to_f(resp[(c + j) * 64 + ft]);
-                outp[(c + j) * 64 + ft] = DT<T>::from_f(rnd<T>(silu_f(g)) * u);
-              }
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float r = __uint_as_float(v[j]) + bias;
-              if (epi == CTS_EPI_GELU) r = gelu_erf(rnd<T>(r));
-              else if (epi == CTS_EPI_RESIDUAL) r = rnd<T>(r) + DT<T>::to_f(resp[(c + j) * kBM + ft]);
-              outp[(c + j) * kBM + ft] = DT<T>::from_f(r);
-            }
-          }
+        for (int i = 0; i < kPBN / 2; ++i) {
+          const float g = rnd<T>(acc.d[0][i]);
+          const float u = rnd<T>(acc.d[1][i]);
+          outp[acc_col(i) * 64 + acc_row(i)] = DT<T>::from_f(rnd<T>(silu_f(g)) * u);
         }
-        if (ch == kPBN / kPChunk - 1) {                   // last TMEM read of this accumulator: hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-        }
-        if (chunk_live) {
-          fence_proxy_async_smem();
-          named_bar_sync(1, 128);
-          if (threadIdx.x == 64) {
-            if (epi == CTS_EPI_SWIGLU_IL) tma_store_2d(&tm_out, out_s, f0 / 2, tc0);
-            else tma_store_2d(&tm_out, out_s, f0, tc0);
-            tma_store_commit();
-            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");     // staging tile may be rewritten
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float bias[2] = {0.f, 0.f};
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const long long f = (long long)f0 + 64 * h + acc_row(2 * e);
+            if (biasp != nullptr && f < p.n) bias[e] = DT<T>::to_f(biasp[f]);
           }
-          named_bar_sync(1, 128);
+#pragma unroll
+          for (int i = 0; i < kPBN / 2; ++i) {
+            const int ft = 64 * h + acc_row(i), tt = acc_col(i);
+            float r = acc.d[h][i] + bias[(i >> 1) & 1];
+            if (epi == CTS_EPI_GELU) r = gelu_erf(rnd<T>(r));
+            else if (epi == CTS_EPI_RESIDUAL) r = rnd<T>(r) + DT<T>::to_f(resp[tt * kBM + ft]);
+            outp[tt * kBM + ft] = DT<T>::from_f(r);
+          }
         }
       }
+      fence_proxy_async_smem();                           // generic-proxy smem writes -> visible to the TMA engine
+      named_bar_sync(1, 128);
+      if (threadIdx.x == 0) {
+        if (epi == CTS_EPI_SWIGLU_IL) tma_store_2d(&tm_out, out_s, f0 / 2, t0);
+        else tma_store_2d(&tm_out, out_s, f0, t0);
+        tma_store_commit();
+        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");     // staging tile may be rewritten
+      }
+      named_bar_sync(1, 128);                             // staging and residual tiles are free again
     }
-    if (threadIdx.x == 64) tma_store_wait_read0();        // all stores fully performed before the CTA retires
+    if (threadIdx.x == 0) tma_store_wait_read0();         // all stores fully performed before the CTA retires
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<512>(tmem_base);
 }
 
 template <typename T>
@@ -532,11 +463,11 @@ int launch_persistent(cts_ctx* ctx, const cts_gemm_args* a, cudaStream_t stream)
   if (rc) return rc;
   rc = cts_make_tmap_2d(ctx, &tm_x, a->x, a->t, a->k, a->x_ld, kPBN, is_bf16);
   if (rc) return rc;
-  rc = cts_make_tmap_2d_dense(ctx, &tm_out, a->out, a->t, il ? a->n / 2 : a->n, a->out_ld, kPChunk, il ? 64 : kBM, is_bf16);
+  rc = cts_make_tmap_2d_dense(ctx, &tm_out, a->out, a->t, il ? a->n / 2 : a->n, a->out_ld, kPBN, il ? 64 : kBM, is_bf16);
   if (rc) return rc;
   tm_res = tm_out;
   if (a->epilogue == CTS_EPI_RESIDUAL) {
-    rc = cts_make_tmap_2d_dense(ctx, &tm_res, a->residual, a->t, a->n, a->out_ld, kPChunk, kBM, is_bf16);
+    rc = cts_make_tmap_2d_dense(ctx, &tm_res, a->residual, a->t, a->n, a->out_ld, kPBN, kBM, is_bf16);
     if (rc) return rc;
   }
   GemmParams p;
@@ -546,9 +477,9 @@ int launch_persistent(cts_ctx* ctx, const cts_gemm_args* a, cudaStream_t stream)
   p.kb_total = (int)cdiv_ll(a->k, kBK);
   p.split_k = 1; p.epilogue = a->epilogue; p.stages = kPStages;
   {
-    // feature tiles per L2 group: keep the group's weights within ~48 MB, balanced over the groups
+    // feature tiles per L2 group: keep the group's weights within ~20 MB (40 % of the H100's 50 MB L2), balanced over the groups
     const long long tiles_m = cdiv_ll(a->n, kBM);
-    long long gmax = (48LL << 20) / ((long long)kBM * a->k * 2);
+    long long gmax = (20LL << 20) / ((long long)kBM * a->k * 2);
     if (gmax < 1) gmax = 1;
     const long long groups = cdiv_ll(tiles_m, gmax);
     p.l2_prefetch = (int)cdiv_ll(tiles_m, groups);       // field reused as "group_m" by the persistent kernel
@@ -577,7 +508,7 @@ int launch(cts_ctx* ctx, const cts_gemm_args* a, cudaStream_t stream) {
   }
   rc = cts_make_tmap_2d(ctx, &tm_x, a->x, a->t, a->k, a->x_ld, BN, is_bf16);
   if (rc) return rc;
-  // big tiles without a row scatter: output (and residual) tiles move by TMA through shared memory
+  // big tiles without a row scatter: output (and residual) tiles move by TMA through shared memory (the ring is idle by then)
   const bool staged = BN >= 64 && a->row_map == nullptr && a->epilogue != CTS_EPI_PARTIAL_F32 && a->epilogue != CTS_EPI_SPLITK_F32 && (a->out_ld * 2) % 16 == 0 &&
                       ((uintptr_t)a->out & 15) == 0 && (a->epilogue != CTS_EPI_RESIDUAL || ((uintptr_t)a->residual & 15) == 0);
   CUtensorMap tm_out = tm_x, tm_res = tm_x;
@@ -628,7 +559,11 @@ int launch(cts_ctx* ctx, const cts_gemm_args* a, cudaStream_t stream) {
     const long long per = ((long long)ctx->l2_prefetch_mb << 20) / (ctas * kBM * kBK * 2 * (DUAL ? 2 : 1));
     p.l2_prefetch = (int)(per > 64 ? 64 : per);
   }
-  const size_t smem = (size_t)stages * kStage + 1024;
+  if (staged && stages * kStage < 2 * BN * kBM * 2) stages = (2 * BN * kBM * 2 + kStage - 1) / kStage;
+  p.stages = stages;
+  const size_t acc_bytes = (size_t)acc_smem_bytes<BN>() * (DUAL ? 2 : 1);
+  const size_t ring = (size_t)stages * kStage;
+  const size_t smem = (acc_in_ring<BN>() ? (ring > acc_bytes ? ring : acc_bytes) : ring + acc_bytes) + 1024;
   auto kern = gemm_tn_kernel<T, BN, DUAL>;
   CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid((unsigned)cdiv_ll(a->n, kBM), (unsigned)cdiv_ll(a->t, BN), (unsigned)a->split_k);
@@ -641,9 +576,9 @@ int dispatch_bn(cts_ctx* ctx, const cts_gemm_args* a, cudaStream_t stream) {
   const long long t = a->t;
   if (t <= 16) return launch<T, 16, DUAL>(ctx, a, stream);
   if (t <= 32) return launch<T, 32, DUAL>(ctx, a, stream);
-  if (t <= 64) return launch<T, 64, DUAL>(ctx, a, stream);
-  if (t <= 128) return launch<T, 128, DUAL>(ctx, a, stream);
-  return launch<T, 256, DUAL>(ctx, a, stream);
+  // one warpgroup holds the whole 128 x BN accumulator in registers: BN <= 128, and <= 64 with the second (w2) accumulator
+  if (t <= 64 || DUAL) return launch<T, 64, DUAL>(ctx, a, stream);
+  return launch<T, 128, false>(ctx, a, stream);
 }
 
 }  // namespace
@@ -686,7 +621,7 @@ extern "C" int cts_gemm(cts_ctx* ctx, const cts_gemm_args* a, void* stream) {
 
 extern "C" int cts_gemm_suggest_split(cts_ctx* ctx, long long n, long long k, long long t, int dual) {
   if (!ctx || n <= 0 || k <= 0 || t <= 0) return 1;
-  const int bn = t <= 16 ? 16 : t <= 32 ? 32 : t <= 64 ? 64 : t <= 128 ? 128 : 256;
+  const int bn = t <= 16 ? 16 : t <= 32 ? 32 : t <= 64 ? 64 : 128;
   // dual = 1: the caller passes n = intermediate size of an INTERLEAVED gate/up weight, whose GEMM has 2 n / 128 tiles; that grid is
   // sized against the three decode CTAs an SM holds (432 of 444 slots at the 14B shape, and one wave again under tensor parallelism,
   // where the old 2-per-SM rule applied to n / 128 tiles gave 540 CTAs = two waves at TP2: csrc/trace.cuh timeline)

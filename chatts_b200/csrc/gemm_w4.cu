@@ -1,18 +1,18 @@
 // chatts_b200 -- W4A16 decode GEMM for the GPTQ-Int4 checkpoints the reference advertises (README.md:52,262-263):
 //     partial[s][t][n] = sum_{k in split s} x[t][k] * sc[n][k / g] * (q[n][k] - zp[n][k / g])        (fp32 accumulate)
 // A decode step is bound by the HBM stream of the weights; 4-bit codes are a quarter of the bf16 bytes (ChatTS-14B: 7 GB per step
-// instead of 28), so the kernel keeps the swap-AB tcgen05 structure of gemm_tn_kernel -- weight tile = the 128-row MMA operand A, the
-// tokens = the MMA N dimension, accumulator in TMEM -- and moves the dequantisation INTO the operand path:
-//   warp 0      TMA producer: packed tiles [128 rows x 32 B] (64 K codes per row) into a deep staging ring (6 x 4 KB in flight
+// instead of 28), so the kernel keeps the swap-AB wgmma structure of gemm_tn_kernel -- weight tile = the 128-row MMA operand A, the
+// tokens = the MMA N dimension, accumulator in registers -- and moves the dequantisation INTO the operand path:
+//   warp 4      TMA producer: packed tiles [128 rows x 32 B] (64 K codes per row) into a deep staging ring (6 x 4 KB in flight
 //               per CTA -- what keeps HBM busy -- requested BEFORE the dependency wait: nobody writes weights)
-//   warps 2..5  work item = one 32-bit word of codes (a row's 8 K elements): int4 -> bf16/fp16 with the magic-number trick (code | 0x4300 is the bf16
+//   warps 5..   work item = one 32-bit word of codes (a row's 8 K elements): int4 -> bf16/fp16 with the magic-number trick (code | 0x4300 is the bf16
 //               128 + code; - (128 + zp), x scale in packed half2 arithmetic = round(scale x (code - zp)) exactly, the value
 //               weights.py:dequantize_gptq_linear(scale_dtype = model dtype) stores for the prefill) -> the 128B-swizzled K-major A tile of an
-//               MMA stage; warp 2 also requests the token tile of that stage; later the same warps run the epilogue
-//   warp 1      tcgen05.mma issuer, as in gemm_tn_kernel
+//               MMA stage; warp 5 also requests the token tile of that stage
+//   warps 0..3  wgmma warpgroup, then the epilogue
 // Split-K partials (CTS_EPI_PARTIAL_F32 semantics): the decode step's reduce kernels finish the projections as they do for bf16
 // weights, so a quantised layer changes ONE launch in the step.  T <= 32 tokens (decode); prefill uses the dequantised copy
-// (180 GB of HBM hold both).  Result: bit-identical to cts_gemm on the dequantised weight (same values, same MMA order).
+// (HBM holds both).  Result: bit-identical to cts_gemm on the dequantised weight (same values, same MMA order).
 #include <type_traits>
 
 #include "common.cuh"
@@ -24,11 +24,12 @@
 
 namespace {
 
-constexpr int kBM = 128, kBK = 64, kUmmaK = 16;
+constexpr int kBM = 128, kBK = 64;
 constexpr int kDqWarps = 8;             // dequantising warps per CTA: the int4 -> 16-bit conversion is instruction-issue bound (ncu: 39 % issue
                                         // active with 4 warps and 1.5 CTAs per SM), so it gets as many warps as the shared memory budget allows CTAs
 constexpr int kDqThreads = kDqWarps * 32;
-constexpr int kThreads = 64 + kDqThreads;
+constexpr int kDq0 = 160;              // first dequantising thread: after the MMA warpgroup and the producer warp
+constexpr int kThreads = kDq0 + kDqThreads;
 constexpr int kStg = 8;                 // staging ring of packed tiles (4 KB each): 48 KB of weight stream in flight per CTA, two CTAs per SM
                                         // (the first runs had 5 slots = 20 KB: the 4-bit stream was latency-bound at ~1.6 TB/s)
 constexpr int kMs = 3;                  // MMA stages (dequantised A tile 16 KB + token tile): the conversion of block i+2 must not wait for the MMA of block i
@@ -68,11 +69,10 @@ template <> struct Magic<__half> {
 };
 
 template <typename T, int BN>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 2)   // two CTAs per SM: the split heuristic below sizes one wave of them
 gemm_w4_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x, const W4Params p) {
   CTS_DYN_SMEM(smem_raw);
-  __shared__ uint64_t stg_full[kStg], stg_empty[kStg], mma_full[kMs], mma_empty[kMs], acc_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t stg_full[kStg], stg_empty[kStg], mma_full[kMs], mma_empty[kMs];
   __shared__ uint16_t sc_s[kMaxGroups][kBM];       // scale bits per (group, row)
   __shared__ uint8_t zp_s[kMaxGroups][kBM];        // integer zero point per (group, row)
 
@@ -100,16 +100,11 @@ gemm_w4_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__
     tma_prefetch_desc(&tm_x);
     for (int s = 0; s < kStg; ++s) { mbar_init(&stg_full[s], 1); mbar_init(&stg_empty[s], kDqWarps); }
     for (int s = 0; s < kMs; ++s) { mbar_init(&mma_full[s], 1 + kDqWarps); mbar_init(&mma_empty[s], 1); }
-    mbar_init(&acc_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<32>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------ TMA producer: the packed weight stream (weights are static: no dependency wait) ------------------------------
     if (lane == 0) {
       CTS_TRACE(CTS_TK_GEMM, 0);
@@ -121,28 +116,32 @@ gemm_w4_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__
       }
       CTS_TRACE(CTS_TK_GEMM, 2);
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(kIsBf16 ? 1 : 0, BN, kBM);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % kMs;
-        mbar_wait(&mma_full[s], ((uint32_t)(i / kMs)) & 1u);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(mma_s + (size_t)s * kMStage);
-        const uint64_t a_desc = umma_desc_k_sw128(a_addr), b_desc = umma_desc_k_sw128(a_addr + kABytes);
-#pragma unroll
-        for (int kk = 0; kk < kBK / kUmmaK; ++kk) {
-          const uint64_t adv = (uint64_t)(kk * ((kUmmaK * 2) >> 4));
-          umma_f16(tmem_base, a_desc + adv, b_desc + adv, idesc, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&mma_empty[s]);
-      }
-      umma_commit(&acc_bar);
+  } else if (warp < 4) {
+    // ------------------------------ MMA warpgroup ------------------------------
+    Acc128<BN> acc;
+    acc.zero();
+    for (int i = 0; i < nkb; ++i) {
+      const int s = i % kMs;
+      mbar_wait(&mma_full[s], ((uint32_t)(i / kMs)) & 1u);
+      const uint32_t a_addr = smem_u32(mma_s + (size_t)s * kMStage);
+      acc.template mma_kblock<kIsBf16>(a_addr, a_addr + kABytes, i == 0);
+      wgmma_wait<1>();
+      if (i > 0 && threadIdx.x == 0) mbar_arrive(&mma_empty[(i - 1) % kMs]);
     }
+    wgmma_wait<0>();
+    if (nkb > 0 && threadIdx.x == 0) mbar_arrive(&mma_empty[(nkb - 1) % kMs]);
+    // ------------------------------ epilogue: fp32 partial of this split ------------------------------
+    float* dst = p.out + (long long)split * p.t * p.n;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) {
+        const long long fo = (long long)f0 + 64 * h + acc_row(i), t = acc_col(i);
+        if (t < p.t && fo < p.n) dst[t * p.n + fo] = acc.d[h][i];
+      }
   } else {
-    // ------------------------------ dequantisers (thread = weight row), then the epilogue ------------------------------
-    const int r = (int)threadIdx.x - 64;                    // 0..kDqThreads-1; the first 128 also own a row of the (group, row) table
+    // ------------------------------ dequantisers (thread = weight row) ------------------------------
+    const int r = (int)threadIdx.x - kDq0;                    // 0..kDqThreads-1; the first 128 also own a row of the (group, row) table
     const long long f = (long long)f0 + r;
     const bool f_ok = f < p.n && r < kBM;
     if (r < kBM) {
@@ -163,12 +162,12 @@ gemm_w4_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__
     }
     named_bar_sync(1, kDqThreads);                          // the (group, row) table is read by other threads than the ones that wrote it
     pdl_wait();                                             // the token operand comes from the predecessor
-    if (threadIdx.x == 64) CTS_TRACE(CTS_TK_GEMM, 1);
+    if (threadIdx.x == kDq0) CTS_TRACE(CTS_TK_GEMM, 1);
     for (int i = 0; i < nkb; ++i) {
       const int ss = i % kStg, ms = i % kMs;
       mbar_wait(&mma_empty[ms], (((uint32_t)(i / kMs)) & 1u) ^ 1u);        // the MMAs that read this stage have completed
       uint8_t* a_tile = mma_s + (size_t)ms * kMStage;
-      if (threadIdx.x == 64) {                                            // the token tile of this stage (L2-resident, evict-last)
+      if (threadIdx.x == kDq0) {                                          // the token tile of this stage (L2-resident, evict-last)
         mbar_expect_tx(&mma_full[ms], (uint32_t)(BN * kBK * 2));
         tma_load_2d(a_tile + kABytes, &tm_x, &mma_full[ms], (kb0 + i) * kBK, 0, CTS_L2_EVICT_LAST);
       }
@@ -176,10 +175,10 @@ gemm_w4_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__
       // Work item = (row, 16-byte output chunk) = ONE 32-bit word of codes: the 32 lanes of a warp take 4 consecutive rows x 8 chunks,
       // so a warp reads 128 contiguous bytes of the packed tile and writes 4 complete 128-byte rows of the swizzled operand tile --
       // both conflict-free (the first version mapped a thread to a whole row: every 16-byte store of a warp hit 32 different rows,
-      // 16 wavefronts each, and the kernel ran at the speed of the shared-memory store pipe: 1.06x over bf16 on the first B200 run).
+      // 16 wavefronts each, and the kernel ran at the speed of the shared-memory store pipe).
       const uint32_t* stg32 = reinterpret_cast<const uint32_t*>(stg_s + (size_t)ss * kPacked);
       const int g = ((kb0 + i) * kBK) / p.group_size - g0;
-      const int wq = warp - 2;                                            // 0..kDqWarps-1
+      const int wq = warp - kDq0 / 32;                                    // 0..kDqWarps-1
       constexpr int kIts = kBM / (4 * kDqWarps);                          // 4 rows per warp and iteration
       uint32_t wv[kIts];
 #pragma unroll
@@ -204,38 +203,8 @@ gemm_w4_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__
         mbar_arrive(&mma_full[ms]);
       }
     }
-    // ------------------------------ epilogue: fp32 partial of this split ------------------------------
-    if (nkb > 0) {
-      mbar_wait(&acc_bar, 0);
-      tc_fence_after();
-    }
-    const int q = warp & 3;                                // TMEM lane quarter this warp may read (32x32b: lanes 32 (warp % 4) ..)
-    const int ch2 = (warp - 2) >> 2;                       // the two warps of a quarter split the token columns
-    const int ft = q * 32 + lane;                          // TMEM lane = output feature
-    const long long fo = (long long)f0 + ft;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    float* dst = p.out + (long long)split * p.t * p.n;
-#pragma unroll 1
-    for (int c = ch2 * 16; c < BN; c += 16 * (kDqWarps / 4)) {
-      if (c >= p.t) break;
-      uint32_t v[16];
-      if (nkb > 0) {
-        tmem_ld_32x32b_x16(lane_addr + (uint32_t)c, v);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0u;
-      }
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const long long t = c + j;
-        if (t < p.t && fo < p.n) dst[t * p.n + fo] = __uint_as_float(v[j]);
-      }
-    }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<32>(tmem_base);
   if (threadIdx.x == 0) CTS_TRACE(CTS_TK_GEMM, 3);
 }
 
@@ -271,7 +240,7 @@ int launch_w4(cts_ctx* ctx, const cts_gemm_w4_args* a, cudaStream_t stream) {
 extern "C" int cts_gemm_w4_suggest_split(cts_ctx* ctx, long long n, long long k) {
   if (!ctx || n <= 0 || k <= 0) return 1;
   const long long tiles = cdiv_ll(n, kBM), kb = cdiv_ll(k, kBK);
-  long long s = (4LL * ctx->sm_count) / tiles;          // ~two waves of the two CTAs an SM holds: measured best (profiles/r2_w4_gemm_*.json)
+  long long s = (4LL * ctx->sm_count) / tiles;          // ~two waves of the two CTAs an SM holds (__launch_bounds__)
   if (s > kb / 2) s = kb / 2;
   if (s > 16) s = 16;
   if (s < 1) s = 1;

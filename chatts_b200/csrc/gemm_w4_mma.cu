@@ -1,9 +1,9 @@
 // chatts_b200 -- W4A16 decode GEMM, register-operand version (GPTQ-Int4 checkpoints, README.md:52,262-263):
 //     partial[s][t][n] = sum_{k in split s} x[t][k] * sc[n][k / g] * (q[n][k] - zp[n][k / g])        (fp32 accumulate)
-// Why a second kernel: gemm_w4.cu keeps the tcgen05 structure and writes the dequantised 16-bit tile to shared memory for the tensor
+// Why a second kernel: gemm_w4.cu keeps the wgmma structure and writes the dequantised 16-bit tile to shared memory for the tensor
 // core to read back; per 128 x 64 block that is 16 KB written + 18 KB read by the MMA + the 4-bit tile in and out = 44 KB through a
 // 128 B/clk shared-memory port, i.e. at most ~24 weights per clock and SM where HBM delivers 46 -- the kernel measured NO faster than
-// the bf16 GEMM (profiles/r2_w4_gemm_tcgen05_final.json).  Here the weight operand never touches shared memory as 16-bit data:
+// the bf16 GEMM.  Here the weight operand never touches shared memory as 16-bit data:
 //   * load-time layout (weights.py:repack_w4_mma): for every (256-feature tile, 64-K block) one contiguous 8 KB chunk whose 32-bit
 //     words ARE the A fragments of mma.sync.m16n8k16 -- lane (g, t) of m-tile j finds, for each of the block's four k16 steps, one
 //     word holding the 8 codes {rows g / g+8} x {k 2t, 2t+1, 2t+8, 2t+9} in the nibble order that `(w >> 4i) & 0x000F000F` turns
@@ -17,15 +17,15 @@
 //     tile; mma.sync with the fp32 accumulators of 2 m-tiles x NT n-tiles in registers
 //   * persistent CTAs over (tile, K split) units, the producers run ahead across unit boundaries
 // What the loop is bound by, measured: instruction issue on the ALU side plus barrier round trips -- 57-59 % issue-active with six warps
-// per scheduler at 64-96 registers, ALU pipe ~50 %, FMA pipe ~25 % (profiles/r2_ncu_w4_mma_summary.json).  Two experiments bracket it:
-//   * rejected (profiles/r2_w4_mma_gemm_sweep_fast.json, git b975740): feeding the MMA the pairs (128 + code) themselves and applying the
+// per scheduler at 64-96 registers, ALU pipe ~50 %, FMA pipe ~25 %.  Two experiments bracket it:
+//   * rejected: feeding the MMA the pairs (128 + code) themselves and applying the
 //     group's scale / zero point in fp32 once per group and accumulator (no HADD2 / HMUL2 per weight, one more MMA per k16 step with an
 //     all-ones A operand for sum_k x_k) removed a quarter of the loop's instructions -- all of them FMA-pipe work that was overlapping for
 //     free -- and was NOT faster (gate_up at t = 1: 26.7 us against 25.8);
 //   * kept: going from 64-K stages on two rings to 128-K stages on one ring halves the waits, arrivals, ring steps and scale fetches per
 //     weight (all ALU / control work): 25.8 -> 19.9 us.
 // Output: the fp32 split-K partials [split, t, n] of CTS_EPI_PARTIAL_F32, so the decode step's reduce tails are unchanged.  The A
-// operand holds the same 16-bit values as the dense copy; the fp32 summation order differs from the tcgen05 GEMM (parity is a
+// operand holds the same 16-bit values as the dense copy; the fp32 summation order differs from the wgmma GEMM (parity is a
 // tolerance, tests/test_gpu_w4.py), unlike gemm_w4.cu which is bit-identical and stays as the checker for this kernel.
 #include <stdlib.h>
 
@@ -298,8 +298,7 @@ gemm_w4_mma_kernel(const __grid_constant__ CUtensorMap tm_x, const W4mParams p) 
 }
 
 // Resident CTAs per SM: three of the t <= 8 kernel (64 registers) when the projection has enough 256-feature tiles to give every CTA a
-// long unit (gate_up: 108 tiles), else two with deeper rings -- measured on a B200: gate_up 28.1 -> 25.8 us with three, down_proj (20
-// tiles) 15.1 -> 18.2 us (profiles/r2_w4_mma_gemm_sweep*.json)
+// long unit (gate_up: 108 tiles), else two with deeper rings
 static inline int w4m_ctas_per_sm(long long tiles, long long t) {
   static const int forced = [] { const char* e = getenv("CTS_W4M_CTAS"); return e ? atoi(e) : 0; }();      // A/B knob (2 or 3)
   if (forced == 2 || (forced == 3 && t <= 8)) return forced;

@@ -6,7 +6,7 @@
 // (tokens x features / tokens x ranks tiles, staged by cp.async, double-buffered):
 //     A[m = feature][k = token] = Ps[token][feature]^T      B[k = token][n = rank] = Qs[token][rank]
 // CTA = 64 features (4 warps x 16) x 16 ranks; grid (ceil(M/64), ceil(r/16), token splits), fp32 atomics across the splits
-// exactly like the FMA kernel.  OPT-IN (CTS_WGRAD_MMA=1) until it has run on a B200; cts_lora_wgrad falls back to the
+// exactly like the FMA kernel.  cts_lora_wgrad falls back to the
 // (validated) FMA kernel whenever a 16-byte alignment precondition does not hold.  No flag / barrier spin.
 #include <stdlib.h>
 
@@ -123,7 +123,7 @@ lora_wgrad_mma_kernel(const T* __restrict__ P, long long p_ld, long long p_col0,
 
 }  // namespace
 
-// Default since round 2 (validated on a B200: equal to the FMA kernel's result, LoRA step 18 % faster, profiles/r2_bench_lora_variants.txt);
+// The default (the GPU tests check it against the FMA kernel's result);
 // CTS_WGRAD_MMA=0 selects the FMA kernel.
 bool cts_lora_wgrad_mma_enabled() {
   const char* e = getenv("CTS_WGRAD_MMA");

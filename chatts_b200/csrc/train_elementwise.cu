@@ -575,7 +575,7 @@ extern "C" int cts_gather_rows(cts_ctx* ctx, const void* src, const int* idx, lo
   return CTS_OK;
 }
 
-// tensor-core variant (lora_wgrad_mma.cu), opt-in through CTS_WGRAD_MMA=1 until it has run on a B200
+// tensor-core variant (lora_wgrad_mma.cu), the default; CTS_WGRAD_MMA=0 selects the FMA kernel
 bool cts_lora_wgrad_mma_enabled();
 bool cts_lora_wgrad_mma_ok(const void* p, long long p_ld, long long p_col0, int p_il, long long m, const void* q, long long q_ld,
                            long long q_col0, int r);

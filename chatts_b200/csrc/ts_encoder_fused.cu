@@ -7,8 +7,8 @@
 // (3 front-end + 5 GEMM + 5 split-K tail launches, 126 us = 0.27 of the HBM roof) pays a kernel boundary per stage.  Here:
 //   * one persistent grid, (hidden/128 feature tiles) x (S K-splits), the S splits of a tile forming one thread-block CLUSTER;
 //   * phase 0: the CTAs assemble the patch rows ([values | position embeddings], 16-byte vector stores) into rows_ws;
-//   * per layer: swap-AB tcgen05 GEMM exactly as gemm_decode_fused.cu (weight tile = the 128-row MMA operand A streamed by TMA with
-//     an evict-first hint, the patch rows = the MMA N dimension, accumulator [128 features x rows] fp32 in TMEM), the split's tile
+//   * per layer: swap-AB wgmma GEMM exactly as gemm_decode_fused.cu (weight tile = the 128-row MMA operand A streamed by TMA with
+//     an evict-first hint, the patch rows = the MMA N dimension, accumulator [128 features x rows] fp32 in registers), the split's tile
 //     parked in shared memory, reduced over DISTRIBUTED SHARED MEMORY in split order, bias + GELU applied, rows written as the next
 //     layer's K-major operand (last layer: scattered through row_map into inputs_embeds);
 //   * between layers a grid barrier (bounded spin -> trap, never a hang) -- and while a CTA waits there its TMA producer already
@@ -31,7 +31,8 @@ namespace {
 
 namespace cg = cooperative_groups;
 
-constexpr int kBM = 128, kBK = 64, kUmmaK = 16, kThreads = 192, kMaxStages = 8;
+// warps 0..7: two MMA warpgroups (the second one only for 256-row tiles: each holds 128 rows of the token tile), warp 8: TMA producer
+constexpr int kBM = 128, kBK = 64, kThreads = 288, kMaxStages = 8;
 constexpr int kTsMaxLayers = 6;
 
 struct alignas(64) TsMaps {
@@ -74,14 +75,14 @@ ts_encoder_fused_kernel(const __grid_constant__ TsMaps maps, const TsFusedParams
   CTS_DYN_SMEM(smem_raw);
   __shared__ uint64_t full_bar[kMaxStages];
   __shared__ uint64_t empty_bar[kMaxStages];
-  __shared__ uint64_t acc_bar;
-  __shared__ uint32_t tmem_slot;
   __shared__ int row_series_s;
 
   constexpr int kABytes = kBM * kBK * 2;
   constexpr int kStage = kABytes + BN * kBK * 2;
   constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
   static_assert(BN == 64 || BN == 128 || BN == 256, "row tile");
+  constexpr int kWN = BN > 128 ? 128 : BN;                  // token rows per MMA warpgroup
+  constexpr int kWGs = BN / kWN;                           // MMA warpgroups
 
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -102,15 +103,10 @@ ts_encoder_fused_kernel(const __grid_constant__ TsMaps maps, const TsFusedParams
   if (threadIdx.x == 0) {
     for (int l = 0; l < p.num_layers; ++l) tma_prefetch_desc(&maps.w[l]);
     for (int i = 0; i < 3; ++i) tma_prefetch_desc(&maps.x[i]);
-    for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&acc_bar, 1);
+    for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kWGs); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<BN < 32 ? 32 : BN>(&tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
   // K range of this CTA's unit in layer l
   auto unit = [&](int l, int& kb0, int& nkb) {
@@ -119,7 +115,7 @@ ts_encoder_fused_kernel(const __grid_constant__ TsMaps maps, const TsFusedParams
     kb0 = (int)(((long long)kb_total * split) / S);
     nkb = (int)(((long long)kb_total * (split + 1)) / S) - kb0;
   };
-  // producer state (lane 0 of warp 0): global iteration counter over every K block of every layer; `pre` = weight tiles of the
+  // producer state (lane 0 of warp 8): global iteration counter over every K block of every layer; `pre` = weight tiles of the
   // current layer already requested before the grid barrier
   int it_p = 0, pre = 0;
   auto issue_weights = [&](int l, int kb0, int from, int upto) {
@@ -160,7 +156,7 @@ ts_encoder_fused_kernel(const __grid_constant__ TsMaps maps, const TsFusedParams
   // The producer may still request layer 0's weight tiles before the dependency wait (nobody writes weights).
   int kb0, nkb;
   unit(0, kb0, nkb);
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     CTS_TRACE(CTS_TK_OTHER, 0);
     pre = nkb < stages ? nkb : stages;
     issue_weights(0, kb0, 0, pre);
@@ -197,12 +193,11 @@ ts_encoder_fused_kernel(const __grid_constant__ TsMaps maps, const TsFusedParams
   grid_barrier();
   if (threadIdx.x == 0) CTS_TRACE(CTS_TK_OTHER, 4);       // rows assembled, layer 0 may start
 
-  uint32_t acc_uses = 0;                                    // completed accumulator phases of THIS CTA (layers with nkb > 0)
   int it_c = 0;                                             // consumer (MMA) iteration counter, mirrors it_p
   for (int l = 0; l < p.num_layers; ++l) {
     unit(l, kb0, nkb);
     const CUtensorMap* tx = &maps.x[l == 0 ? 0 : 1 + ((l - 1) & 1)];
-    if (warp == 0) {
+    if (warp == 8) {
       // ------------------------------ TMA producer ------------------------------
       if (lane == 0) {
         for (int i = 0; i < pre; ++i) {                     // token tiles of the stages whose weight tile is already on its way
@@ -222,71 +217,54 @@ ts_encoder_fused_kernel(const __grid_constant__ TsMaps maps, const TsFusedParams
         pre = 0;
         CTS_TRACE(CTS_TK_OTHER, 5);                         // this layer's last load requested
         // This CTA's stream of layer l is fully requested: pull ITS unit of layer l + 1 into L2 now (fire-and-forget), so HBM keeps
-        // streaming through the drain, the cluster barrier, the DSMEM tail and the grid barrier (~10 us per layer on the first B200
-        // timeline -- as long as a whole layer's 52 MB stream); a layer is 52 MB, the L2 126 MB, and nothing else streams meanwhile.
+        // streaming through the drain, the cluster barrier, the DSMEM tail and the grid barrier; the prefetched lines are the ones
+        // this CTA itself reads next, and nothing else streams meanwhile.
         if (l + 1 < p.num_layers) {
           int kb0n, nkbn;
           unit(l + 1, kb0n, nkbn);
           for (int i = 0; i < nkbn; ++i) tma_prefetch_l2_2d(&maps.w[l + 1], (kb0n + i) * kBK, f0);
         }
       }
-    } else if (warp == 1) {
-      // ------------------------------ MMA issuer ------------------------------
-      if (lane == 0) {
-        constexpr uint32_t idesc = umma_idesc_f16(kIsBf16 ? 1 : 0, BN, kBM);
-        for (int i = 0; i < nkb; ++i) {
-          const int it = it_c + i;
-          const int s = it % stages;
-          mbar_wait(&full_bar[s], ((uint32_t)(it / stages)) & 1u);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
-          const uint64_t a_desc = umma_desc_k_sw128(a_addr), b_desc = umma_desc_k_sw128(a_addr + kABytes);
-#pragma unroll
-          for (int kk = 0; kk < kBK / kUmmaK; ++kk) {
-            const uint64_t adv = (uint64_t)(kk * ((kUmmaK * 2) >> 4));
-            umma_f16(tmem_base, a_desc + adv, b_desc + adv, idesc, (i > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        if (nkb > 0) umma_commit(&acc_bar);
-        it_c += nkb;
+    } else if (warp < 4 * kWGs) {
+      // ------------------------------ MMA warpgroup(s) ------------------------------
+      const int wg = warp >> 2;
+      const bool wg_lead = (threadIdx.x & 127) == 0;
+      Acc128<kWN> acc;
+      acc.zero();
+      for (int i = 0; i < nkb; ++i) {
+        const int it = it_c + i;
+        const int s = it % stages;
+        mbar_wait(&full_bar[s], ((uint32_t)(it / stages)) & 1u);
+        const uint32_t a_addr = smem_u32(smem + (size_t)s * kStage);
+        acc.template mma_kblock<kIsBf16>(a_addr, a_addr + kABytes + wg * kWN * 128, i == 0);
+        wgmma_wait<1>();
+        if (i > 0 && wg_lead) mbar_arrive(&empty_bar[(it - 1) % stages]);
       }
-    } else {
-      // ------------------------------ epilogue, part A: park this split's fp32 tile in shared memory ------------------------------
-      if (nkb > 0) {
-        mbar_wait(&acc_bar, acc_uses & 1u);
-        tc_fence_after();
-      }
+      wgmma_wait<0>();
+      if (nkb > 0 && wg_lead) mbar_arrive(&empty_bar[(it_c + nkb - 1) % stages]);
+      it_c += nkb;
       if (threadIdx.x == 64) CTS_TRACE(CTS_TK_OTHER, 6);    // accumulator complete
-      const int q = warp & 3;
-      const int ft = q * 32 + lane;
-      const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 16) {
-        if (c >= R) break;                                  // warp-uniform
-        uint32_t v[16];
-        if (nkb > 0) {
-          tmem_ld_32x32b_x16(lane_addr + (uint32_t)c, v);
-          tmem_ld_wait();
-        } else {
+      // ------------------------------ epilogue, part A: park this split's fp32 tile in shared memory ------------------------------
+      named_bar_sync(1, 128 * kWGs);                        // every warp's MMAs are done with the ring
 #pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = 0u;
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < kWN / 2; ++i) {
+          const int c = wg * kWN + acc_col(i);
+          if (c < R) part_s[c * kBM + 64 * h + acc_row(i)] = acc.d[h][i];
         }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) part_s[(c + j) * kBM + ft] = __uint_as_float(v[j]);
-      }
-      tc_fence_before();
+    } else {
+      it_c += nkb;                                          // idle warps keep the (unused) counter in step
     }
-    if (nkb > 0) ++acc_uses;                                // CTA-uniform bookkeeping (every thread keeps its own copy)
     __syncthreads();
     cluster.sync();                                         // every split's tile is in its CTA's shared memory
     if (threadIdx.x == 64) CTS_TRACE(CTS_TK_OTHER, 7);
 
-    if (warp >= 2) {
+    if (warp >= 2 && warp < 6) {                          // the 128 threads part B is written for (et = 0..127)
       // ------------------------------ epilogue, part B: rows r = split, split + S, ...: reduce over DSMEM in split order, apply the tail ------------------------------
       // Work item = (one of this CTA's rows, 4 consecutive features): S 16-byte loads from the peers' parked tiles, issued for TWO items
-      // before the first add (the first B200 timeline showed a scalar, one-row-at-a-time tail costing 17 us per layer -- DSMEM round
-      // trips, not arithmetic), then bias + GELU on four values and ONE 8-byte store.
+      // before the first add (a scalar, one-row-at-a-time tail pays a DSMEM round trip per row), then bias + GELU on four values and
+      // ONE 8-byte store.
       const int et = (int)threadIdx.x - 64;                  // 0..127
       const bool last = l + 1 == p.num_layers;
       const T* bias_p = reinterpret_cast<const T*>(p.bias[l]);
@@ -352,9 +330,7 @@ ts_encoder_fused_kernel(const __grid_constant__ TsMaps maps, const TsFusedParams
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<BN < 32 ? 32 : BN>(tmem_base);
   pdl_trigger();
   if (threadIdx.x == 0) {
     CTS_TRACE(CTS_TK_OTHER, 3);
@@ -407,7 +383,7 @@ int launch_ts_fused(cts_ctx* ctx, const cts_ts_encode_args* a, int* sync, cudaSt
   auto kern = ts_encoder_fused_kernel<T, BN>;
   CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 #ifndef CTS_HOST_SHIM
-  // without the maximum carve-out the driver places ONE 97 KB CTA per SM (first B200 run: 120 resident CTAs, split 3)
+  // without the maximum carve-out the driver may place only ONE CTA per SM
   CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
 #endif
   const int tiles = (int)cdiv_ll(a->hidden, kBM);
@@ -418,9 +394,7 @@ int launch_ts_fused(cts_ctx* ctx, const cts_ts_encode_args* a, int* sync, cudaSt
 #ifdef CTS_HOST_SHIM
   S = kb_max < 4 ? kb_max : 4;
 #else
-  // The driver's cluster-occupancy query counts ONE CTA of this kernel per SM on a B200 (first runs: 148 single-CTA clusters, 45 of
-  // size 3) although two fit by every resource (97 KB of shared memory, 108 registers x 192 threads, 2 x 128 TMEM columns) and 240
-  // CTAs in clusters of 6 do run co-resident.  Sound bound from what the query does answer: the SMs that hold a cluster of c CTAs
+  // The driver's cluster-occupancy query may count ONE CTA of this kernel per SM although two fit by every resource.  Sound bound from what the query does answer: the SMs that hold a cluster of c CTAs
   // at one CTA per SM hold a cluster of 2c at two per SM, so  clusters(2c at 2/SM) >= clusters(c at 1/SM).
   auto api_clusters = [&](int c) {
     cudaLaunchConfig_t q = {};
@@ -443,7 +417,7 @@ int launch_ts_fused(cts_ctx* ctx, const cts_ts_encode_args* a, int* sync, cudaSt
   CTS_CUDA(ctx, cudaFuncGetAttributes(&fattr, kern));
   const long long smem_cta = (long long)smem + (long long)fattr.sharedSizeBytes + 1024;
   const long long regs_cta = (long long)((fattr.numRegs + 7) / 8 * 8) * kThreads;
-  const bool two_fit = per_sm_api >= 2 || (2 * smem_cta <= 227LL * 1024 && 2 * regs_cta <= 65536 && 2 * BN <= 512 && 2 * kThreads <= 2048);
+  const bool two_fit = per_sm_api >= 2 || (2 * smem_cta <= 227LL * 1024 && 2 * regs_cta <= 65536 && 2 * kThreads <= 2048);
   for (int cand = 8; cand >= 1 && S == 0; --cand) {
     if (cand > kb_max) continue;
     if (api_clusters(cand) >= tiles) { S = cand; break; }

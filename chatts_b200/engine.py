@@ -1,4 +1,4 @@
-"""Iteration-level ("continuous") batching over the B200 decode step (SURVEY.md 8(f) N3; what the reference gets from vLLM's
+"""Iteration-level ("continuous") batching over the decode step (SURVEY.md 8(f) N3; what the reference gets from vLLM's
 scheduler, chatts/utils/llm_utils.py:147-190 / vllm_stream_qa.py:34-59).
 
 The decode step of ``ChatTSForCausalLM`` is one CUDA graph over STATIC per-slot state (current id, position, sequence

@@ -1,13 +1,13 @@
-"""ChatTSForCausalLM on B200: TS encoder -> merge at ``<ts>`` -> Qwen2 decoder -> lm_head, behind the
+"""ChatTSForCausalLM on H100: TS encoder -> merge at ``<ts>`` -> Qwen2 decoder -> lm_head, behind the
 ``generate()`` surface the reference's callers use (README.md:88-103, demo/demo_hf.ipynb cells 3-5,
 chatts/utils/inference_tsmllm_deepspeed.py:89-106).
 
 Replaces, for this path only: the checkpoint's remote-code ``Qwen2TSForCausalLM`` (HF surface) and
-``chatts.vllm.chatts_vllm.Qwen2TSForCausalLM`` (chatts_vllm.py:452-625).  All arithmetic runs in the sm_100a
+``chatts.vllm.chatts_vllm.Qwen2TSForCausalLM`` (chatts_vllm.py:452-625).  All arithmetic runs in the sm_90a
 kernels of libchatts_b200.so; torch provides device memory, streams, CUDA-graph capture and
-torch.distributed.  There is no CPU or eager-torch fallback: constructing the model without a B200 raises.
+torch.distributed.  There is no CPU or eager-torch fallback: constructing the model without an H100 raises.
 
-Decode is a single CUDA graph per batch size: embedding gather -> [split-K tcgen05 GEMM -> fused
+Decode is a single CUDA graph per batch size: embedding gather -> [split-K wgmma GEMM -> fused
 reduce(+bias+RoPE+KV write | +residual+RMSNorm | SwiGLU)] x layers -> paged flash-decode -> lm_head -> argmax
 -> device-side advance (next id, position, KV slot), so a step replays with no host round trip.
 """
@@ -67,7 +67,7 @@ class ChatTSForCausalLM:
                  max_batch=32, max_seq_len=2048, page_size=64, use_cuda_graph=True, comm=None,
                  use_peer_allreduce=True, graph_with_tp=True, use_chain=None, use_sample_kernel=None, use_native_step=None, use_fused_decode=None, use_peer_ll=None):
         if not torch.cuda.is_available():
-            raise _cabi.CtsError("chatts_b200 needs a B200 (sm_100a) GPU; there is no CPU fallback")
+            raise _cabi.CtsError("chatts_b200 needs an H100 (sm_90a) GPU; there is no CPU fallback")
         self.config, self.dtype = config, dtype
         self.device = torch.device(device if str(device) != "cuda" else f"cuda:{torch.cuda.current_device()}")
         self.tp_rank, self.tp_size, self.comm = tp_rank, tp_size, comm
@@ -86,17 +86,16 @@ class ChatTSForCausalLM:
         import os as _os
         self.use_chain = bool(int(_os.environ.get("CTS_DECODE_CHAIN", "0"))) if use_chain is None else bool(use_chain)
         # the whole decode step enqueued by one C call (cts_decoder_step) instead of ~440 ctypes calls: identical launches; off by
-        # default until compared with the Python orchestration on a B200 (CTS_NATIVE_STEP=1 / use_native_step=True)
+        # default (CTS_NATIVE_STEP=1 / use_native_step=True)
         self.use_native_step = bool(int(_os.environ.get("CTS_NATIVE_STEP", "0"))) if use_native_step is None else bool(use_native_step)
         # decode GEMMs with the split-K reduction and the projection tail fused in through a thread-block cluster
-        # (csrc/gemm_decode_fused.cu: 9 -> 7 dependent stages per layer); off by default until it has run on a B200
+        # (csrc/gemm_decode_fused.cu: 9 -> 7 dependent stages per layer); off by default
         #   1: projections fused with their tails, plain RMSNorm launches between them (7 stages, bit-identical to the default path)
         #   2: the RMSNorms too -- the residual projections emit per-tile sums of squares, the next projection builds its normalised
         #      token operand itself (5 stages; single GPU only)
         self.use_fused_decode = int(_os.environ.get("CTS_DECODE_FUSED", "0")) if use_fused_decode is None else int(use_fused_decode)
         # tensor parallelism: low-latency two-shot all-reduce (cts_peer_allreduce_ll) instead of the one-shot push kernel
-        # (default since round 2: validated across 2 B200s -- same logits, same tokens on every rank -- and 19-25 % faster per step
-        #  than the one-shot kernel at TP2, profiles/r2_tp2_variants.txt; CTS_PEER_LL=0 selects the one-shot kernel)
+        # (the default: same logits, same tokens on every rank; CTS_PEER_LL=0 selects the one-shot kernel)
         self.use_peer_ll = (_os.environ.get("CTS_PEER_LL", "1") == "1") if use_peer_ll is None else bool(use_peer_ll)
         # row-parallel exchange of prefill-sized steps: "rs_ag" (default: fp32 reduce-scatter + 16-bit all-gather of the result), "fp32"
         # (one fp32 all-reduce, rounds 1-2), "16bit" (all-reduce in the model dtype: vLLM's semantics, fastest, re-rounds the running sum)
@@ -108,13 +107,11 @@ class ChatTSForCausalLM:
             except Exception:
                 self._nccl = False
         # sampled decoding through cts_sample_advance (csrc/sampling.cu): temperature / top-k / top-p / multinomial / advance in ONE
-        # launch per step, no torch op on the path (validated on a B200: 17 cases against the CPU statement that is itself checked
-        # against transformers' logits warpers).  Default since round 2; CTS_SAMPLE_KERNEL=0 selects the torch-op fallback.
+        # launch per step, no torch op on the path (checked against a CPU statement that is itself checked
+        # against transformers' logits warpers).  The default; CTS_SAMPLE_KERNEL=0 selects the torch-op fallback.
         self.use_sample_kernel = bool(int(_os.environ.get("CTS_SAMPLE_KERNEL", "1"))) if use_sample_kernel is None else bool(use_sample_kernel)
-        # bytes of the NEXT GEMM's weight a decode GEMM prefetches into L2 once its own stream is requested.  OFF by default: measured
-        # on a B200 (profiles/r2_next_prefetch_ab.txt) it fills the gaps between the weight streams but makes the step SLOWER
-        # (b=32: 6.59 ms without, 6.83 / 7.00 / 7.08 ms with 24 / 48 / 80 MB) -- the prefetched lines do not survive the current
-        # GEMM's stream through L2, so the bytes are read twice.  CTS_NEXT_PREFETCH_MB=<n> turns it on for experiments.
+        # bytes of the NEXT GEMM's weight a decode GEMM prefetches into L2 once its own stream is requested.  OFF by default: the
+        # prefetched lines do not survive the current GEMM's stream through L2, so the bytes are read twice.  CTS_NEXT_PREFETCH_MB=<n> turns it on for experiments.
         self.next_prefetch_bytes = int(float(_os.environ.get("CTS_NEXT_PREFETCH_MB", "0")) * (1 << 20))
         self.w4 = None               # W4A16 decode weights (csrc/gemm_w4.cu): set by attach_w4 / quantize_w4_synthetic / from_pretrained(GPTQ)
         self._load(state_dict)
@@ -280,7 +277,7 @@ class ChatTSForCausalLM:
         """Switch the DECODE step to the 4-bit weight stream.  ``packed``: {HF linear name (e.g. 'model.layers.3.mlp.up_proj'):
         (qw uint8 [out, in/2], scales [out, in/g], zeros uint8 [out, in/g])} in the layout of weights.py:repack_gptq_w4, for all
         seven projections of every layer.  The dense weights stay (prefill and every T > 32 step use them): they must hold the SAME
-        values, i.e. weights.py:dequantize_gptq(..., scale_dtype=model dtype) -- 180 GB of HBM keep both copies.  Fused operands
+        values, i.e. weights.py:dequantize_gptq(..., scale_dtype=model dtype) -- HBM keeps both copies.  Fused operands
         are assembled exactly like the dense ones: q|k|v stacked, gate/up interleaved per 64 rows.  Single GPU (a tensor-parallel
         row split would cut groups: down_proj's 13824 / 8 = 1728 inputs are not a multiple of the group size)."""
         if self.tp_size != 1:
@@ -307,12 +304,12 @@ class ChatTSForCausalLM:
         c = self.ctx
         import os as _os
         # kernel of the decode step: "mma" (default) = csrc/gemm_w4_mma.cu, the codes dequantised in registers from the fragment-major copy
-        # built here (the row layout is dropped per layer once it is converted); "tc5" = csrc/gemm_w4.cu (tcgen05, bit-identical to the
+        # built here (the row layout is dropped per layer once it is converted); "tc5" = csrc/gemm_w4.cu (wgmma, bit-identical to the
         # dense GEMM, no faster than it: kept as the checker)
         w4["kernel"] = _os.environ.get("CTS_W4_KERNEL", "mma")
         k_dims = (self.H, self.nh * self.d, self.I)
         if w4["kernel"] == "mma" and not (all(kd % 128 == 0 for kd in k_dims) and (gs == 64 or gs % 128 == 0)):
-            w4["kernel"] = "tc5"          # the mma kernel's pipeline stage is 128 K wide (cts_gemm_w4f_args): odd shapes take the tcgen05 kernel
+            w4["kernel"] = "tc5"          # the mma kernel's pipeline stage is 128 K wide (cts_gemm_w4f_args): odd shapes take the wgmma kernel
         if w4["kernel"] == "mma":
             from .weights import repack_w4_mma
             for kind in ("qkv", "o", "gu", "d"):
@@ -507,9 +504,8 @@ class ChatTSForCausalLM:
         big = split == 1 and not (self.peer is not None and T <= self.peer_tokens)
         if big and self.tp_prefill_exchange == "16bit":
             # Opt-in (CTS_TP_PREFILL_EXCHANGE=16bit): every rank rounds its projection to the model dtype and NCCL sums the ranks' outputs
-            # in that dtype -- what vLLM's RowParallelLinear does (qwen2.py:100-116 / 168-174) -- half the bytes of the fp32 all-reduce:
-            # e2e at TP4 1 850 -> 2 466 tok/s, and the prefill logits move from 1.2e-2 to 1.8e-2 of max from the single-GPU model
-            # (profiles/r2_bench_tp4_prefill_exchange_*.json).  Not the default: the sum is re-rounded at every ring step.
+            # in that dtype -- what vLLM's RowParallelLinear does (qwen2.py:100-116 / 168-174) -- half the bytes of the fp32 all-reduce.
+            # Not the default: the sum is re-rounded at every ring step, which moves the logits further from the single-GPU model.
             proj = st.tp_proj
             c.gemm(x, w, proj, epilogue=EPI_NONE, t=T)
             torch.distributed.all_reduce(proj[:T], group=self.comm)

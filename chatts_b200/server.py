@@ -1,4 +1,4 @@
-"""OpenAI-style HTTP front end for the B200 engine (SURVEY.md 8(f) N3): what ``scripts/start_vllm_server.sh`` +
+"""OpenAI-style HTTP front end for the native engine (SURVEY.md 8(f) N3): what ``scripts/start_vllm_server.sh`` +
 ``demo/vllm_api.py`` give a ChatTS user -- ``POST /v1/chat/completions`` whose user message carries text parts and
 ``{"timeseries": [...]}`` parts, consumed in ``<ts><ts/>`` order (demo/vllm_api.py:45-55) -- plus ``/v1/completions`` with the
 vLLM request shape (``prompt`` + ``multi_modal_data.timeseries``, demo/demo_vllm.py:47-52), ``/v1/models`` and ``/health``.

@@ -1,4 +1,4 @@
-"""LoRA fine-tune step of the ChatTS decoder on B200 (SURVEY.md 8(a) row A9, BASELINE config 5: ChatTS-8B, forward +
+"""LoRA fine-tune step of the ChatTS decoder (BASELINE config 5: ChatTS-8B, forward +
 backward on ``{input, output, timeseries}`` records, data parallel).
 
 What the reference gives for this row: nothing executable -- training lives in the external ChatTS-Training project
@@ -13,9 +13,9 @@ checked against ``oracle/lora.py`` (torch.autograd over the decoder oracle, itse
   * ``clip_grad_norm_`` + ``torch.optim.AdamW`` on fp32 master adapters; gradients are summed across the data-parallel
     ranks with ONE all-reduce of the flat gradient arena (NCCL on the GPUs, gloo in the CPU tests).
 
-B200-first layout (DESIGN.md section 7):
-  * every matrix product is ``cts_gemm`` (tcgen05): the frozen projections, their input gradients dX = dY W through
-    TRANSPOSED copies of the frozen weights that stay resident in HBM (8B: +15 GB of the 180 GB), and the LoRA products,
+Layout:
+  * every matrix product is ``cts_gemm`` (wgmma): the frozen projections, their input gradients dX = dY W through
+    TRANSPOSED copies of the frozen weights that stay resident in HBM (8B: +15 GB), and the LoRA products,
     which are fused per projection GROUP -- qkv / o / gate_up / down -- into two small GEMMs: U = X A_f^T with the member
     A's stacked ([R, K], R = r x members) and Y += U B_f^T with the member B's block-placed in [N, R] (alpha/r folded in);
   * the skinny weight gradients dB = s dY^T U and dA = dU^T X stream dY / X once (``cts_lora_wgrad``, HBM-bound) straight

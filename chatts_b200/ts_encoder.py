@@ -1,6 +1,6 @@
-"""Value-Preserved Time-Series Encoder on B200 -- host mirror of ``TimeSeriesEmbedding``
+"""Value-Preserved Time-Series Encoder on H100 -- host mirror of ``TimeSeriesEmbedding``
 (chatts/vllm/chatts_vllm.py:61-193): same constructor config, same ``forward(x) -> (feats, patch_cnt)``
-contract, same error behaviour; the arithmetic runs in the sm_100a kernels behind the C-ABI
+contract, same error behaviour; the arithmetic runs in the sm_90a kernels behind the C-ABI
 (cts_ts_patch_count, cts_ts_patchify, cts_gemm [+ cts_reduce_bias_act]).
 
 One device->host copy of N int32 pairs per call (valid_len, patch_cnt) replaces the reference's 2-3 syncs

@@ -3,7 +3,7 @@ chatts/utils/llm_utils.py:147-190): ``LLM(model=...).generate([{"prompt": str, "
 {"timeseries": [...]}}], SamplingParams(...)) -> outputs[i].outputs[0].text``.
 
 The reference's plugin file targets vllm 0.8.5 internals that no longer exist (SURVEY.md §8b); this shim
-keeps the REQUEST SHAPE and drives the B200 engine directly instead of vLLM's plugin ABI."""
+keeps the REQUEST SHAPE and drives the native engine directly instead of vLLM's plugin ABI."""
 from dataclasses import dataclass, field
 
 import numpy as np

@@ -128,7 +128,7 @@ def dequantize_gptq_linear(qweight, qzeros, scales, g_idx=None, group_size=128, 
     return w.t().contiguous().to(dtype)
 
 
-# nibble position of K element j (0..7) inside a 32-bit word of the B200 layout: ((w >> 4 i) & 0x000F000F) yields the pair
+# nibble position of K element j (0..7) inside a 32-bit word of the fragment-major layout: ((w >> 4 i) & 0x000F000F) yields the pair
 # (k_2i, k_2i+1) in the low / high half-word, i.e. one 16-bit-pair per shift -- the form the magic-number int4 -> bf16/fp16
 # conversion wants (csrc/gemm_w4.cu)
 W4_NIBBLE_OF_K = (0, 4, 1, 5, 2, 6, 3, 7)

@@ -1,4 +1,4 @@
-/* chatts_b200 -- C-ABI of the B200 (sm_100a) hot path of ChatTS.
+/* chatts_b200 -- C-ABI of the H100 (sm_90a) hot path of ChatTS.
  *
  * The reference (NetManAIOps/ChatTS @ 09fae34) has NO native boundary for this path: it is Python on
  * top of torch / vLLM / transformers.  This header is the boundary a maintainer binds from Python with
@@ -32,7 +32,7 @@ extern "C" {
 
 typedef struct cts_ctx cts_ctx;
 
-/* library identity: cts_arch() must say "sm_100a". */
+/* library identity: cts_arch() must say "sm_90a". */
 int cts_version(void);
 const char* cts_arch(void);
 
@@ -66,12 +66,12 @@ int cts_ts_patchify(cts_ctx* ctx, const void* x, int dtype, int n_series, int ro
                     void* rows_out, int in0, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * tcgen05 GEMM  Y[T, N] = X[T, K] * W[N, K]^T  (+ fused epilogue)
+ * wgmma GEMM  Y[T, N] = X[T, K] * W[N, K]^T  (+ fused epilogue)
  *   replaces nn.Linear in  TimeSeriesEmbedding.mlp (chatts_vllm.py:83-91,188) and every projection of the
  *   decoder (transformers qwen2/modeling_qwen2.py:44-48,217-219,245; vllm qwen2.py:93-116,159-174;
  *   lm_head chatts_vllm.py:607-610).
  *   Weights stream through TMA as the 128-row MMA operand, tokens are the MMA N dimension ("swap-AB"), so
- *   decode batches of 1..32 tokens still issue full-width tcgen05.mma and the kernel is HBM-bound on W.
+ *   decode batches of 1..32 tokens still fill the 128 rows of the wgmma tile and the kernel is HBM-bound on W.
  */
 #define CTS_EPI_NONE 0        /* out = dtype(acc + bias)                                      */
 #define CTS_EPI_GELU 1        /* out = dtype(gelu_erf(dtype(acc + bias)))      chatts_vllm.py:86-87 */
@@ -160,7 +160,7 @@ int cts_embed_gather(cts_ctx* ctx, const void* table, const int* ids, void* out,
  * K8 attention                       modeling_qwen2.py:161-184 ; vllm qwen2.py:188-197,234
  * prefill: causal GQA over the tokens of this call, variable length, cu_seqlens int32[batch+1]
  *   q [t, nh, d], k/v [t, nkv, d] (RoPE applied), out [t, nh*d]; total_tokens = t (rows of q/k/v; bounds the TMA maps)
- *   head_dim 128: tcgen05 kernel (TMA-staged Q/K/V, S and O accumulators in TMEM); head_dim 64: HMMA (wmma) kernel
+ *   head_dim 128: wgmma kernel (TMA-staged Q/K/V, S and O accumulators in registers); head_dim 64: HMMA (wmma) kernel
  */
 int cts_attn_prefill(cts_ctx* ctx, const void* q, const void* k, const void* v, const int* cu_seqlens, int batch,
                      int max_seqlen, long long total_tokens, int nh, int nkv, int head_dim, float scale, void* out,
@@ -357,7 +357,7 @@ int cts_ts_encode(cts_ctx* ctx, const cts_ts_encode_args* args, void* stream);
 
 /* The same encoder as ONE launch (csrc/ts_encoder_fused.cu) for prompts of up to 256 patch rows -- the BASELINE.json metric prompt is
  * 8 series x 256 points = 128 rows: patchify + last-value pad + position-embedding gather (chatts_vllm.py:107-183), every MLP layer
- * (tcgen05, the K splits of a 128-feature tile reduced over distributed shared memory inside a thread-block cluster, bias + exact-erf
+ * (wgmma, the K splits of a 128-feature tile reduced over distributed shared memory inside a thread-block cluster, bias + exact-erf
  * GELU, chatts_vllm.py:83-91,186-188) and the row scatter into inputs_embeds (chatts_vllm.py:569-573), grid barriers between the
  * layers, the next layer's weight tiles requested while a CTA waits.  HBM-bound on the weight stream (212 MB at the 14B shape).
  * valid_len / row_offset / max_valid are INPUTS (cts_ts_patch_count ran: the host sizes the merged sequence from the counts);
@@ -497,7 +497,7 @@ int cts_lora_pack(cts_ctx* ctx, const float* master, const long long* desc, int 
                   int dtype, void* stream);
 
 /* W4A16 decode GEMM for GPTQ-Int4 checkpoints (README.md:52,262-263): partial[s][t][n] = sum over split s of x[t][k] * W[n][k] with
- * W[n][k] = scales[n][k / g] * (q[n][k] - zeros[n][k / g]) dequantised inside the TMA -> shared memory -> tcgen05 operand path
+ * W[n][k] = scales[n][k / g] * (q[n][k] - zeros[n][k / g]) dequantised inside the TMA -> shared memory -> wgmma operand path
  * (csrc/gemm_w4.cu), so a decode step streams the 4-bit codes -- a quarter of the bf16 bytes.  1 <= t <= 32; out = fp32 split-K
  * partials [split_k, t, n] exactly as cts_gemm(CTS_EPI_PARTIAL_F32) writes them (the cts_reduce_* / cts_qkv_rope_cache tails finish
  * the projection); results are bit-identical to cts_gemm on the dequantised weight.

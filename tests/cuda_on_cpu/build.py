@@ -8,13 +8,13 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "chatts_b200", "csrc")
-SOURCES = ["sampling.cu", "train_elementwise.cu", "allreduce_ll.cu", "attention_bwd.cu", "gemm_decode_fused.cu", "gemm_tcgen05.cu", "attention_bwd_tc5.cu", "lora_wgrad_mma.cu", "attention.cu", "elementwise.cu", "ts_frontend.cu", "decoder_step.cu", "allreduce.cu", "ts_encoder_fused.cu", "gemm_w4.cu", "gemm_w4_mma.cu"]
+SOURCES = ["sampling.cu", "train_elementwise.cu", "allreduce_ll.cu", "attention_bwd.cu", "attention_bwd_wgmma.cu", "gemm_decode_fused.cu", "gemm_tcgen05.cu", "lora_wgrad_mma.cu", "attention.cu", "elementwise.cu", "ts_frontend.cu", "decoder_step.cu", "allreduce.cu", "ts_encoder_fused.cu", "gemm_w4.cu", "gemm_w4_mma.cu"]
 OUT = os.path.join(HERE, "_build", "libchatts_shim.so")
 # Files that are GPU-validated are not edited for the shim's sake (not even a spelling): their two non-portable spellings are replaced
 # in the COPY.  Everything else in the copy is the product source, byte for byte.
 _CP16 = '"cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "r"(sz) : "memory");'
 SUBSTITUTIONS = {
-    # the pre-Blackwell warp-level instructions: cp.async is a copy, ldmatrix / mma.sync go to the fragment-exact emulation of common.cuh
+    # the warp-level instructions: cp.async is a copy, ldmatrix / mma.sync go to the fragment-exact emulation of common.cuh
     "lora_wgrad_mma.cu": [
         ("asm volatile(" + _CP16, "if (valid) memcpy(smem, gmem, 16); else memset(smem, 0, 16); (void)sz;"),
         ('asm volatile("cp.async.commit_group;" ::: "memory");', ""),
@@ -43,9 +43,11 @@ SUBSTITUTIONS = {
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));''',
          "{ const uint32_t a_[4] = {a0, a1, a2, a3}; shim_mma_m16n8k16(c, a_, b0, b1, false); }"),
         ("extern __shared__ __align__(128) uint8_t pf_smem[];", "uint8_t* pf_smem = g_dyn_smem;"),
-        ("extern __shared__ uint8_t tc_raw[];", "uint8_t* tc_raw = g_dyn_smem;"),
         ("extern __shared__ uint8_t dec_raw[];", "uint8_t* dec_raw = g_dyn_smem;"),
+        ("extern __shared__ uint8_t wg_raw[];", "uint8_t* wg_raw = g_dyn_smem;"),
     ],
+    "attention_bwd_wgmma.cu": [("extern __shared__ uint8_t bq_raw[];", "uint8_t* bq_raw = g_dyn_smem;"),
+                               ("extern __shared__ uint8_t bkv_raw[];", "uint8_t* bkv_raw = g_dyn_smem;")],
     "elementwise.cu": [("    ss_cta = v;\n  }\n  cluster.sync();", "    ss_cta = v;\n    shim_publish_static(&ss_cta);\n  }\n  cluster.sync();"),
                        ("*cluster.map_shared_rank(&ss_cta, r)", "*(float*)shim_static_peer((unsigned)r)")],
     "allreduce.cu": [
@@ -70,8 +72,6 @@ SUBSTITUTIONS = {
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));''',
          "shim_mma_m16n8k16(c, a, b0, b1, false);"),
     ],
-    "attention_bwd_tc5.cu": [("extern __shared__ uint8_t dq_raw[];", "uint8_t* dq_raw = g_dyn_smem;"),
-                             ("extern __shared__ uint8_t dkv_raw[];", "uint8_t* dkv_raw = g_dyn_smem;")],
     "gemm_tcgen05.cu": [("extern __shared__ uint8_t smem_raw[];", "uint8_t* smem_raw = g_dyn_smem;"),
                         ('asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");', "tma_store_wait_read0();")],
 }

@@ -4,7 +4,7 @@
 // vector types, launch_pdl -- with the execution model
 //     one OS thread per CUDA thread, the threads of ONE block at a time, blocks of a grid one after the other,
 // and the library's own host helpers (cts_ctx, error macros, DT<>, rnd, pack8, warp_sum ...) restated for the host.  The KERNEL
-// BODIES and the C-ABI entry points are the product's, untouched: what runs here is the same source nvcc compiles for sm_100a,
+// BODIES and the C-ABI entry points are the product's, untouched: what runs here is the same source nvcc compiles for sm_90a,
 // which turns "this kernel has never executed" into "its source executes and passes its GPU test on CPU" for the kernels that need
 // no tensor core, TMA or cluster (sampling, AdamW / clip / adapter packing, the elementwise backward kernels, the LL all-reduce).
 // Not a performance model, not a memory-model checker (x86 is stronger than PTX), never part of the product.
@@ -263,7 +263,7 @@ static inline const char* cudaGetErrorString(int) { return "shim"; }
 struct cts_ctx {
   int device;
   int sm_count;
-  int decode_stages, l2_prefetch_mb, no_persistent_gemm, force_wmma_attention, norm_cluster, max_smem_optin;
+  int decode_stages, l2_prefetch_mb, no_persistent_gemm, norm_cluster, max_smem_optin;
   int no_next_prefetch, next_prefetch_mb, no_ts_fused;
   void* scratch;                                           // zero-initialised counters (grid barrier of the fused TS encoder)          // next-GEMM L2 prefetch hint (a no-op on the host: tma_prefetch_l2_2d does nothing)
   char err[512];
@@ -317,12 +317,12 @@ static inline float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.707
 static inline float silu_f(float x) { return x / (1.0f + expf(-x)); }
 
 // ================================================================================================================================
-// Functional emulation of the Blackwell pieces the tensor-core kernels use: mbarrier (arrive / expect_tx / complete_tx / parity wait),
-// TMA tile loads and stores (128-byte swizzle or dense boxes, zero fill / clipping at the tensor edge), TMEM (128 lanes x 512 fp32
-// columns per CTA), tcgen05.mma kind::f16 with cta_group::1 (shared-memory matrix descriptors decoded: K-major and MN-major operands,
-// 128-byte swizzle applied on the ADDRESS bits as the hardware does), tcgen05.ld 32x32b and tcgen05.commit.  Everything completes
-// synchronously at issue, so this checks what the kernels COMPUTE and that their barrier protocols are live, not asynchrony hazards.
-// The semantics encoded here are calibrated by running the GPU-validated kernels of gemm_tcgen05.cu through them.
+// Functional emulation of the Hopper pieces the tensor-core kernels use: mbarrier (arrive / expect_tx / complete_tx / parity wait),
+// TMA tile loads and stores (128-byte swizzle or dense boxes, zero fill / clipping at the tensor edge) and the warpgroup MMA of the
+// swap-AB GEMMs (Acc128: shared-memory matrix descriptors decoded, 128-byte swizzle applied on the ADDRESS bits as the hardware does,
+// every thread computing its own registers of the documented m64nNk16 accumulator fragment).  The MMA completes synchronously at
+// issue (CTS_SHIM_ASYNC delays TMA loads / stores only), so this checks what the kernels COMPUTE and that their barrier protocols
+// are live, not MMA-completion hazards.
 // ================================================================================================================================
 #include <unordered_map>
 // 32-bit shared-window addresses: the low half of the host pointer; the high half is remembered per CTA (all shared objects a kernel
@@ -332,11 +332,11 @@ static inline uint32_t smem_u32(const void* p) { g_smem_hi = (uint64_t)(uintptr_
 static inline uint8_t* shim_smem_from_u32(uint32_t a) { return (uint8_t*)(uintptr_t)((g_smem_hi << 32) | a); }
 struct CUtensorMap { const void* base; long long rows, cols, ld; int box_rows, box_cols, swizzled, is_bf16; };
 
-// CTS_SHIM_ASYNC=1 -- adversarially LATE completion of the asynchronous operations: a TMA load / store, a tcgen05.mma and the arrive of a
-// tcgen05.commit are queued at issue and performed (in issue order) only when some thread of the CTA is blocked in an mbarrier wait or
-// in one of the explicit completion waits, and at the latest when the CTA ends.  A consumer that reads shared memory, TMEM or global
-// memory without having waited for the producing operation, or a producer that overwrites an operand buffer an outstanding MMA has not
-// read yet, then sees stale or clobbered data and its test fails.  (Off: everything completes at issue.)
+// CTS_SHIM_ASYNC=1 -- adversarially LATE completion of the TMA loads and stores: they are queued at issue and performed (in issue order)
+// only when some thread of the CTA is blocked in an mbarrier wait or in one of the explicit completion waits, and at the latest when the
+// CTA ends.  A consumer that reads shared or global memory without having waited for the producing copy, or a producer that refills a
+// slot before its consumers released it, then sees stale or clobbered data and its test fails.  The warpgroup MMAs complete at issue.
+// (Off: everything completes at issue.)
 #include <deque>
 extern thread_local std::deque<std::function<void()>> g_async;
 extern int g_async_mode;
@@ -395,12 +395,6 @@ static inline void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes
   shim_async([=] { memcpy(smem_dst, gsrc, bytes); shim_mbar_complete_tx(bar, bytes); });
 }
 static inline bool elect_one() { return (shim_linear_tid() & 31) == 0; }
-static inline void tc_fence_before() {}
-static inline void tc_fence_after() {}
-
-extern thread_local float g_tmem[128][512];
-template <int kCols> static inline void tmem_alloc(uint32_t* smem_slot) { *smem_slot = 0; }
-template <int kCols> static inline void tmem_dealloc(uint32_t) {}
 static inline uint8_t* shim_smem_ptr(uint32_t addr18) {                           // 18-bit shared-window address -> this CTA's dynamic shared memory
   return g_dyn_smem + ((addr18 - ((uint32_t)(uintptr_t)g_dyn_smem & 0x3FFFFu)) & 0x3FFFFu);
 }
@@ -412,52 +406,88 @@ static inline float shim_ld_elem(const uint8_t* p, bool bf16) {
 // operand element (r, k): r = row of A (M) or of B (N); major 0 = K-major (rows of 128 B), 1 = MN-major (the r index is contiguous)
 static inline float shim_operand(uint64_t desc, int major, int r, int k, bool bf16) {
   const uint32_t start = (uint32_t)(desc & 0x3FFF) << 4, lbo = (uint32_t)((desc >> 16) & 0x3FFF) << 4, sbo = (uint32_t)((desc >> 32) & 0x3FFF) << 4;
-  if (((desc >> 61) & 7) != 2) { printf("shim: only SWIZZLE_128B shared-memory descriptors are emulated\n"); __trap(); }
+  if (((desc >> 62) & 3) != 1) { printf("shim: only SWIZZLE_128B shared-memory descriptors are emulated\n"); __trap(); }
   const uint8_t* base = shim_smem_ptr(start);
   const size_t off = major == 0 ? (size_t)(r / 8) * sbo + (size_t)(r % 8) * 128 + (size_t)k * 2
                                 : (size_t)(r / 64) * lbo + (size_t)(k / 8) * sbo + (size_t)(k % 8) * 128 + (size_t)(r % 64) * 2;
   return shim_ld_elem(base + off, bf16);
 }
-static inline void shim_umma_now(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  const int N = (int)((idesc >> 17) & 0x3F) << 3, M = (int)((idesc >> 24) & 0x1F) << 4;
-  const int a_major = (int)((idesc >> 15) & 1), b_major = (int)((idesc >> 16) & 1);
-  const bool bf16 = ((idesc >> 7) & 7) == 1;
-  if (M != 128) { printf("shim: tcgen05.mma with M = %d is not emulated\n", M); __trap(); }
-  const int lane0 = (int)(d_tmem >> 16), col0 = (int)(d_tmem & 0xFFFF);
-  static thread_local float A[128][16], B[256][16];
-  for (int m = 0; m < M; ++m)
-    for (int k = 0; k < 16; ++k) A[m][k] = shim_operand(a_desc, a_major, m, k, bf16);
-  for (int n = 0; n < N; ++n)
-    for (int k = 0; k < 16; ++k) B[n][k] = shim_operand(b_desc, b_major, n, k, bf16);
-  for (int m = 0; m < M; ++m)
-    for (int n = 0; n < N; ++n) {
-      float acc = accumulate ? g_tmem[lane0 + m][col0 + n] : 0.f;
-      for (int k = 0; k < 16; ++k) acc += A[m][k] * B[n][k];
-      g_tmem[lane0 + m][col0 + n] = acc;
+static inline uint64_t gmma_desc_k_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+static inline void wgmma_fence() {}
+static inline void wgmma_commit() {}
+template <int N> static inline void wgmma_wait() {}
+static inline int acc_row(int i) { return ((shim_linear_tid() >> 5) & 3) * 16 + ((shim_linear_tid() & 31) >> 2) + ((i >> 1) & 1) * 8; }
+static inline int acc_col(int i) { return (i >> 2) * 8 + (shim_linear_tid() & 3) * 2 + (i & 1); }
+static inline float shim_half_of(uint32_t word, int half, bool bf16);
+static inline uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) |
+         ((uint64_t)1 << 62);
+}
+static inline void wgmma_fence_operand(float&) {}
+// m64nNk16, both operands K-major in shared memory: every thread computes its own accumulator registers
+template <int N, bool BF16> static inline void wgmma_m64k16(float* d, uint64_t a, uint64_t b, int scale_d) {
+  for (int i = 0; i < N / 2; ++i) {
+    float acc = scale_d ? d[i] : 0.f;
+    for (int k = 0; k < 16; ++k) acc += shim_operand(a, 0, acc_row(i), k, BF16) * shim_operand(b, 0, acc_col(i), k, BF16);
+    d[i] = acc;
+  }
+}
+// m64n128k16 with A in registers (the warpgroup's fragments are gathered through a per-CTA table) and B MN-major
+template <bool BF16> static inline void wgmma_m64n128k16_rs_tb(float* d, const uint32_t* a, uint64_t b) {
+  static thread_local uint32_t ga[128][4];
+  const int tl = shim_linear_tid() & 127;
+  for (int e = 0; e < 4; ++e) ga[tl][e] = a[e];
+  named_bar_sync(14, 128);
+  auto A = [&](int row, int k) {                 // a0: (g, 2t..) a1: (g+8, 2t..) a2: (g, 2t+8..) a3: (g+8, 2t+8..) of warp row / 16
+    const int owner = (row / 16) * 32 + (row % 8) * 4 + (k % 8) / 2, e = ((row % 16) >= 8 ? 1 : 0) + (k >= 8 ? 2 : 0);
+    return shim_half_of(ga[owner][e], k % 2, BF16);
+  };
+  for (int i = 0; i < 64; ++i) {
+    float acc = d[i];
+    for (int k = 0; k < 16; ++k) acc += A(acc_row(i), k) * shim_operand(b, 1, acc_col(i), k, BF16);
+    d[i] = acc;
+  }
+  named_bar_sync(14, 128);
+}
+template <int BN> struct Acc128 {
+  float d[2][BN / 2];
+  void zero() { for (int h = 0; h < 2; ++h) for (int i = 0; i < BN / 2; ++i) d[h][i] = 0.f; }
+  template <bool BF16> void mma_kblock(uint32_t a_addr, uint32_t b_addr, bool first) {
+    // the operand rows this thread's registers touch, decoded once per K block: 2 x 2 rows of A, BN / 4 rows of B
+    float A[2][2][64], B[BN / 4][64];
+    const uint64_t b = gmma_desc_k_sw128(b_addr);
+    for (int j = 0; j < BN / 4; ++j)
+      for (int kk = 0; kk < 4; ++kk)
+        for (int k = 0; k < 16; ++k) B[j][16 * kk + k] = shim_operand(b + 2 * kk, 0, acc_col((j >> 1) * 4 + (j & 1)), k, BF16);
+    for (int h = 0; h < 2; ++h) {
+      const uint64_t a = gmma_desc_k_sw128(a_addr + 64 * 128 * h);
+      for (int r = 0; r < 2; ++r)
+        for (int kk = 0; kk < 4; ++kk)
+          for (int k = 0; k < 16; ++k) A[h][r][16 * kk + k] = shim_operand(a + 2 * kk, 0, acc_row(2 * r), k, BF16);
     }
-}
-static inline void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  shim_async([=] { shim_umma_now(d_tmem, a_desc, b_desc, idesc, accumulate); });
-}
-static inline void umma_commit(uint64_t* bar) { shim_async([=] { mbar_arrive(bar); }); }      // arrives once the MMAs issued before it have been performed
-static inline void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* v) {
-  const int lane = (int)(taddr >> 16) + (shim_linear_tid() & 31), col = (int)(taddr & 0xFFFF);
-  for (int j = 0; j < 16; ++j) v[j] = shim_f2u(g_tmem[lane][col + j]);
-}
-static inline void tmem_ld_wait() {}                     // completes the LOADS only: outstanding MMAs are not performed here
-static inline void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t* v) {
-  const int lane = (int)(taddr >> 16) + (shim_linear_tid() & 31), col = (int)(taddr & 0xFFFF);
-  for (int j = 0; j < 16; ++j) g_tmem[lane][col + j] = shim_u2f(v[j]);
-}
-static inline void tmem_st_wait() {}
-static inline uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-constexpr uint32_t umma_idesc_f16(int is_bf16, int n, int m) {
-  return (1u << 4) | ((uint32_t)(is_bf16 ? 1 : 0) << 7) | ((uint32_t)(is_bf16 ? 1 : 0) << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+    for (int h = 0; h < 2; ++h)
+      for (int i = 0; i < BN / 2; ++i) {
+        const float* ar = A[h][(i >> 1) & 1];
+        const float* br = B[(i >> 2) * 2 + (i & 1)];
+        float acc = first ? 0.f : d[h][i];
+        for (int k = 0; k < 64; ++k) acc += ar[k] * br[k];
+        d[h][i] = acc;
+      }
+  }
+  void store(float* s, int ld) const {
+    for (int h = 0; h < 2; ++h)
+      for (int i = 0; i < BN / 2; ++i) s[(64 * h + acc_row(i)) * ld + acc_col(i)] = d[h][i];
+  }
+};
+template <int BN> constexpr int acc_ld() { return BN + 8; }
+template <int BN> constexpr int acc_smem_bytes() { return 128 * acc_ld<BN>() * 4; }
+static inline void acc_ld16(const float* s, int ld, int row, int col, uint32_t* v) {
+  for (int j = 0; j < 16; ++j) v[j] = shim_f2u(s[row * ld + col + j]);
 }
 
-// ---- warp-level matrix instructions of the pre-Blackwell path (ldmatrix, mma.sync m16n8k16), emulated over the fibers of a warp:
+// ---- warp-level matrix instructions (ldmatrix, mma.sync m16n8k16), emulated over the fibers of a warp:
 // every lane publishes its operands, then computes its own result registers from the documented fragment layouts
 static inline void shim_warp_allgather(uint64_t v, uint64_t* out) {
   ShimBlock::Warp& w = g_blk.warp[shim_linear_tid() >> 5];

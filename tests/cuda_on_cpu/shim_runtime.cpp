@@ -9,7 +9,6 @@ thread_local std::deque<std::function<void()>> g_async;
 int g_async_mode = 0;
 thread_local void* g_static_self = nullptr;
 thread_local std::unordered_map<const void*, ShimMbar> g_mbar;
-thread_local float g_tmem[128][512];
 thread_local uint8_t* g_dyn_smem = nullptr;
 thread_local size_t g_dyn_bytes = 0;
 thread_local bool g_whole_grid_next = false;
@@ -218,7 +217,6 @@ extern "C" int cts_ctx_create(int device, cts_ctx** out) {
   c->decode_stages = 96;
   c->l2_prefetch_mb = 0;
   c->no_persistent_gemm = 0;
-  c->force_wmma_attention = 0;
   c->norm_cluster = 8;
   c->no_next_prefetch = 0;
   c->next_prefetch_mb = 0;

@@ -1,4 +1,4 @@
-"""Schedule-level statement of csrc/attention_bwd.cu (HMMA, 64-row CTAs) and csrc/attention_bwd_tc5.cu (tcgen05, 128-row CTAs) on CPU: the CTA / warp / tile loops, causal and length masks, lse / delta
+"""Schedule-level statement of csrc/attention_bwd.cu (HMMA) and csrc/attention_bwd_wgmma.cu (wgmma), both 64-row CTAs, on CPU: the CTA / warp / tile loops, causal and length masks, lse / delta
 staging and the GQA accumulation order of the two backward kernels, restated line by line in numpy (not the wmma fragment
 addressing, which mirrors the GPU-validated forward kernel) and checked against torch.autograd over the eager attention of
 transformers qwen2/modeling_qwen2.py:161-184.  It pins the ALGORITHM the kernels implement: a wrong tile bound or mask in
@@ -23,8 +23,9 @@ def ref(q,k,v,do,cu,nh,nkv,d):
         o[a:e]=out.detach().numpy(); lse[a:e]=torch.logsumexp(w,-1).T.detach().numpy()
     return dq,dk,dv,o,lse
 def emul(q,k,v,do,o,lse,cu,nh,nkv,d,max_seqlen,BIG=64,SMALL=64):
-    """BIG = rows owned by a CTA, SMALL = rows of the streamed tile: (64, 64) = attention_bwd.cu (4 warps x 16 rows),
-    (128, 64) = attention_bwd_tc5.cu (thread = row)."""
+    """BIG = rows owned by a CTA, SMALL = rows of the streamed tile: (64, 64) = attention_bwd.cu (4 warps x 16 rows) and
+    attention_bwd_wgmma.cu (one warpgroup, m64 fragments); (128, 64) = 128-row CTAs, which no kernel uses: it checks that the result
+    of the schedule does not depend on the CTA height (the causal tile ranges and the GQA order are stated per row, not per CTA)."""
     NW=BIG//16
     scale=1/math.sqrt(d); LOG2E=1.4426950408889634; sl2=scale*LOG2E
     T=q.shape[0]; delta=(o.reshape(T,nh,d)*do.reshape(T,nh,d)).sum(-1)

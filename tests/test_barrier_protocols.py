@@ -1,17 +1,18 @@
-"""Protocol-level simulation of the mbarrier pipelines that have not run on a B200 yet: the tcgen05 attention backward
-(csrc/attention_bwd_tc5.cu: dQ and dK/dV kernels) and the cluster-fused decode GEMM with the in-kernel RMSNorm operand
-(csrc/gemm_decode_fused.cu, NORM_IN).  Each warp role is transcribed as a coroutine that performs the kernel's waits, arrivals,
-TMA issues, tcgen05.mma issues / commits and shared-memory / TMEM reads and writes in the kernel's order; a random scheduler
-interleaves the roles and completes the asynchronous operations (TMA copies, MMAs in issue order) at random later points.
+"""Protocol-level simulation of the mbarrier / wgmma pipelines of the Hopper kernels: the swap-AB GEMM ring (csrc/gemm_tcgen05.cu,
+decode_chain.cu, gemm_decode_fused.cu incl. NORM_IN, ts_encoder_fused.cu, gemm_w4.cu), the wgmma prefill attention
+(csrc/attention.cu) and the wgmma attention backward (csrc/attention_bwd_wgmma.cu: dQ and dK/dV kernels).  The TMA producer and
+the MMA warpgroup are transcribed as coroutines that perform the kernel's waits, arrivals, TMA issues, wgmma issues / commit
+groups / wgmma_wait<N> and shared-memory writes in the kernel's order; a random scheduler interleaves them and completes the
+asynchronous operations (TMA copies in any order, wgmma groups in issue order) at random later points.
 
 What it checks, over many random schedules:
   * liveness -- every role terminates (a lost arrival or a wrong phase parity shows up as a deadlock);
-  * every MMA reads the operand tiles it is meant to read, at issue time AND at completion time (a tile refilled too early, or
-    not yet filled, is a label mismatch);
-  * every TMEM / shared buffer read by the softmax warps holds the tile it is meant to hold.
+  * every MMA reads the operand tiles it is meant to read, at issue time AND at completion time (a slot refilled too early --
+    released before the wgmma group that reads it has been waited for -- or not yet filled, is a label mismatch);
+  * the accumulator chain: every MMA adds to the result of the previous one.
 
 mbarrier semantics modelled: arrival count, expect_tx / complete_tx byte accounting, phase parity with try_wait(parity)
-(a fresh barrier passes a wait on parity 1).  tcgen05.commit arrives when all previously issued MMAs have completed.
+(a fresh barrier passes a wait on parity 1).  wgmma_wait<N> returns once at most N committed groups are outstanding.
 TEST INFRASTRUCTURE ONLY -- it pins the synchronisation design, not the data path.
 """
 import random
@@ -61,7 +62,7 @@ class Sim:
 
     def mma(self, reads, write=None, chain=()):
         """reads: [(buffer, expected label)], write: (buffer, label).  Shared-memory operands are checked now and again at
-        completion; ``chain`` = the accumulator this MMA adds to (TMEM): the tensor core executes MMAs in issue order, so that
+        completion; ``chain`` = the accumulator this MMA adds to: the tensor core executes MMAs in issue order, so that
         dependency is checked at completion only."""
         for b, lab in reads:
             assert self.mem.get(b) == lab, f"MMA issued while {b} holds {self.mem.get(b)}, wanted {lab}"
@@ -70,8 +71,17 @@ class Sim:
     def commit(self, bar):
         self.mma_queue.append(("commit", bar, None))
 
+    def group(self):
+        """wgmma.commit_group: the MMAs issued since the previous group form one group."""
+        self.mma_queue.append(("group", None, None))
+
+    def groups_pending(self):
+        return sum(1 for kind, _, _ in self.mma_queue if kind == "group")
+
     def _step_mma(self):
         kind, a, b = self.mma_queue.pop(0)
+        if kind == "group":
+            return
         if kind == "commit":
             a.arrive()
             return
@@ -115,179 +125,122 @@ def wait(bar, parity):
     return lambda: bar.ready(parity)
 
 
-# ====================================================================================================================== dQ kernel
-def sim_dq(nt, seed):
+def wgmma_wait(s, n):
+    return lambda: s.groups_pending() <= n
+
+
+# ====================================================================================================================== swap-AB GEMM ring
+def sim_gemm_ring(nkb, stages, seed, norm_in=False):
+    """Producer: weight tile (and, unless NORM_IN, the token tile) of K block i into slot i % stages once the slot is released.
+    MMA warpgroup: per block -- (NORM_IN: write the token tile into the slot itself) -- wait full, issue, commit a group,
+    wgmma_wait<1>, release the PREVIOUS block's slot; after the loop wgmma_wait<0> and release the last slot."""
     s = Sim(seed)
-    qdo, kv_full, kv_empty = MBar(1), [MBar(1), MBar(1)], [MBar(1), MBar(1)]            # K/V ring of two stages
-    s_full, s_free, ds_full, ds_free, o_done = MBar(1), MBar(4), MBar(4), MBar(1), MBar(1)
-    s.mem.update({"Q": None, "dO": None, "K0": None, "V0": None, "K1": None, "V1": None, "dS": None, "S": None, "dP": None,
-                  "dQ": ("dQ", -1)})
-
-    def producer():
-        qdo.expect_tx(4)
-        for b in ("Q", "Q", "dO", "dO"):
-            s.tma(b, b, qdo, 1)
-        for j in range(nt):
-            st = j & 1
-            yield wait(kv_empty[st], ((j >> 1) & 1) ^ 1)
-            kv_full[st].expect_tx(4)
-            s.tma(f"K{st}", ("K", j), kv_full[st], 2)
-            s.tma(f"V{st}", ("V", j), kv_full[st], 2)
-            yield None
-
-    def mma():
-        yield wait(qdo, 0)
-        for j in range(nt):
-            st = j & 1
-            yield wait(kv_full[st], (j >> 1) & 1)
-            if j > 0:
-                yield wait(s_free, (j - 1) & 1)
-            s.mma([("Q", "Q"), (f"K{st}", ("K", j))], ("S", ("S", j)))
-            s.mma([("dO", "dO"), (f"V{st}", ("V", j))], ("dP", ("dP", j)))
-            s.commit(s_full)
-            yield wait(ds_full, j & 1)
-            s.mma([("dS", ("dS", j)), (f"K{st}", ("K", j))], ("dQ", ("dQ", j)), chain=[("dQ", ("dQ", j - 1))])
-            s.commit(kv_empty[st])
-            s.commit(ds_free)
-            yield None
-        s.commit(o_done)
-
-    def softmax(w):
-        def g():
-            for j in range(nt):
-                yield wait(s_full, j & 1)
-                assert s.mem["S"] == ("S", j) and s.mem["dP"] == ("dP", j), (s.mem["S"], s.mem["dP"], j)
-                yield None
-                s_free.arrive()
-                if j > 0:
-                    yield wait(ds_free, (j - 1) & 1)
-                s.mem["dS"] = ("dS", j) if w == 3 else s.mem["dS"]      # the tile is complete once the last warp has written
-                yield None
-                ds_full.arrive()
-            yield wait(o_done, 0)
-            assert s.mem["dQ"] == ("dQ", nt - 1)
-        return g()
-
-    s.spawn("tma", producer())
-    s.spawn("mma", mma())
-    for w in range(4):
-        s.spawn(f"softmax{w}", softmax(w))
-    s.run()
-
-
-# ====================================================================================================================== dK/dV kernel
-def sim_dkv(n_iter, seed):
-    s = Sim(seed)
-    kv_bar, qd_full, qd_empty = MBar(1), [MBar(1), MBar(1)], [MBar(1), MBar(1)]          # Q/dO ring of two stages
-    s_full, s_free, pd_full, pd_free, done = MBar(1), MBar(4), MBar(4), MBar(1), MBar(1)
-    s.mem.update({"K": None, "V": None, "Q0": None, "dO0": None, "Q1": None, "dO1": None, "PT": None, "dST": None, "ST": None, "dPT": None,
-                  "dV": ("dV", -1), "dK": ("dK", -1)})
-
-    def producer():
-        kv_bar.expect_tx(2)
-        s.tma("K", "K", kv_bar, 1)
-        s.tma("V", "V", kv_bar, 1)
-        for n in range(n_iter):
-            st = n & 1
-            yield wait(qd_empty[st], ((n >> 1) & 1) ^ 1)
-            qd_full[st].expect_tx(2)
-            s.tma(f"Q{st}", ("Q", n), qd_full[st], 1)
-            s.tma(f"dO{st}", ("dO", n), qd_full[st], 1)
-            yield None
-
-    def mma():
-        yield wait(kv_bar, 0)
-        for n in range(n_iter):
-            st = n & 1
-            yield wait(qd_full[st], (n >> 1) & 1)
-            if n > 0:
-                yield wait(s_free, (n - 1) & 1)
-            s.mma([("K", "K"), (f"Q{st}", ("Q", n))], ("ST", ("ST", n)))
-            s.mma([("V", "V"), (f"dO{st}", ("dO", n))], ("dPT", ("dPT", n)))
-            s.commit(s_full)
-            yield wait(pd_full, n & 1)
-            s.mma([("PT", ("PT", n)), (f"dO{st}", ("dO", n))], ("dV", ("dV", n)), chain=[("dV", ("dV", n - 1))])
-            s.mma([("dST", ("dST", n)), (f"Q{st}", ("Q", n))], ("dK", ("dK", n)), chain=[("dK", ("dK", n - 1))])
-            s.commit(qd_empty[st])
-            s.commit(pd_free)
-            yield None
-        s.commit(done)
-
-    def softmax(w):
-        def g():
-            for n in range(n_iter):
-                yield wait(s_full, n & 1)
-                assert s.mem["ST"] == ("ST", n) and s.mem["dPT"] == ("dPT", n)
-                yield None
-                s_free.arrive()
-                if n > 0:
-                    yield wait(pd_free, (n - 1) & 1)
-                if w == 3:
-                    s.mem["PT"], s.mem["dST"] = ("PT", n), ("dST", n)
-                yield None
-                pd_full.arrive()
-            yield wait(done, 0)
-            assert s.mem["dV"] == ("dV", n_iter - 1) and s.mem["dK"] == ("dK", n_iter - 1)
-        return g()
-
-    s.spawn("tma", producer())
-    s.spawn("mma", mma())
-    for w in range(4):
-        s.spawn(f"softmax{w}", softmax(w))
-    s.run()
-
-
-# ====================================================================================================================== fused decode GEMM, NORM_IN
-def sim_fused_norm_in(nkb, stages, seed):
-    s = Sim(seed)
-    full = [MBar(5) for _ in range(stages)]               # weight tile (expect_tx arrival) + four B-producer warps
-    empty = [MBar(1) for _ in range(stages)]
-    acc = MBar(1)
+    full, empty = [MBar(1) for _ in range(stages)], [MBar(1) for _ in range(stages)]
     for st in range(stages):
         s.mem[f"A{st}"], s.mem[f"B{st}"] = None, None
     s.mem["acc"] = ("acc", -1)
 
     def producer():
-        npre = min(nkb, stages)
-        for i in range(npre):
-            full[i].expect_tx(1)
-            s.tma(f"A{i}", ("A", i), full[i], 1)
-        yield None                                        # pdl_wait
-        for i in range(npre, nkb):
+        for i in range(nkb):
             st = i % stages
             yield wait(empty[st], ((i // stages) & 1) ^ 1)
-            full[st].expect_tx(1)
+            full[st].expect_tx(1 if norm_in else 2)
             s.tma(f"A{st}", ("A", i), full[st], 1)
+            if not norm_in:
+                s.tma(f"B{st}", ("B", i), full[st], 1)
             yield None
 
     def mma():
         for i in range(nkb):
             st = i % stages
+            if norm_in:                                   # slot st was last read by block i - stages: waited for below
+                s.mem[f"B{st}"] = ("B", i)
+                yield None                                # named barrier of the four warps
             yield wait(full[st], (i // stages) & 1)
             s.mma([(f"A{st}", ("A", i)), (f"B{st}", ("B", i))], ("acc", ("acc", i)), chain=[("acc", ("acc", i - 1))])
-            s.commit(empty[st])
+            s.group()
+            yield wgmma_wait(s, 1)
+            if i > 0:
+                empty[(i - 1) % stages].arrive()
             yield None
-        s.commit(acc)
-
-    def bwarp(w):
-        def g():
-            yield None                                    # pdl_wait, rstd staging
-            for i in range(nkb):
-                st = i % stages
-                yield wait(empty[st], ((i // stages) & 1) ^ 1)
-                if w == 3:
-                    s.mem[f"B{st}"] = ("B", i)
-                yield None
-                full[st].arrive()
-            yield wait(acc, 0)
-            assert s.mem["acc"] == ("acc", nkb - 1)
-        return g()
+        yield wgmma_wait(s, 0)
+        if nkb > 0:
+            empty[(nkb - 1) % stages].arrive()
+        assert s.mem["acc"] == ("acc", nkb - 1)
 
     s.spawn("tma", producer())
     s.spawn("mma", mma())
-    for w in range(4):
-        s.spawn(f"bwarp{w}", bwarp(w))
     s.run()
+
+
+# ====================================================================================================================== attention kernels
+def sim_attention(n, fixed, ring, phase1, phase2, seed, acc_names):
+    """The wgmma attention kernels: `fixed` tiles land once on one barrier, `ring` tiles per item on a two-stage ring.  Per item the
+    warpgroup issues the phase-1 MMAs (both operands in shared memory: S / dP), waits for them (wgmma_wait<0>), runs the softmax in
+    registers, issues the phase-2 MMAs (register A operand, a ring tile as B: O, dQ, dV, dK) into the accumulators, waits again and
+    only then releases the ring slot."""
+    s = Sim(seed)
+    fix, full, empty = MBar(1), [MBar(1), MBar(1)], [MBar(1), MBar(1)]
+    for f in fixed:
+        s.mem[f] = None
+    for st in range(2):
+        for r in ring:
+            s.mem[f"{r}{st}"] = None
+    for a in acc_names:
+        s.mem[a] = (a, -1)
+
+    def tile(name, st):
+        return name if name in fixed else f"{name}{st}"
+
+    def label(name, j):
+        return name if name in fixed else (name, j)
+
+    def producer():
+        fix.expect_tx(len(fixed))
+        for f in fixed:
+            s.tma(f, f, fix, 1)
+        for j in range(n):
+            st = j & 1
+            yield wait(empty[st], ((j >> 1) & 1) ^ 1)
+            full[st].expect_tx(len(ring))
+            for r in ring:
+                s.tma(f"{r}{st}", (r, j), full[st], 1)
+            yield None
+
+    def mma():
+        yield wait(fix, 0)
+        for j in range(n):
+            st = j & 1
+            yield wait(full[st], (j >> 1) & 1)
+            for x, y in phase1:
+                s.mma([(tile(x, st), label(x, j)), (tile(y, st), label(y, j))])
+            s.group()
+            yield wgmma_wait(s, 0)
+            yield None                                    # softmax / dS in registers
+            for b_op, acc in phase2:
+                s.mma([(tile(b_op, st), label(b_op, j))], (acc, (acc, j)), chain=[(acc, (acc, j - 1))])
+            s.group()
+            yield wgmma_wait(s, 0)
+            empty[st].arrive()
+            yield None
+        for acc in acc_names:
+            assert s.mem[acc] == (acc, n - 1)
+
+    s.spawn("tma", producer())
+    s.spawn("mma", mma())
+    s.run()
+
+
+def sim_dq(nt, seed):
+    sim_attention(nt, ["Q", "dO"], ["K", "V"], [("Q", "K"), ("dO", "V")], [("K", "dQ")], seed, ["dQ"])
+
+
+def sim_dkv(n_iter, seed):
+    sim_attention(n_iter, ["K", "V"], ["Q", "dO"], [("K", "Q"), ("V", "dO")], [("dO", "dV"), ("Q", "dK")], seed, ["dV", "dK"])
+
+
+def sim_fused_norm_in(nkb, stages, seed):
+    sim_gemm_ring(nkb, stages, seed, norm_in=True)
 
 
 @pytest.mark.parametrize("nt", [1, 2, 3, 6])
@@ -308,44 +261,48 @@ def test_fused_decode_norm_in_pipeline(nkb, stages):
         sim_fused_norm_in(nkb, stages, seed)
 
 
+@pytest.mark.parametrize("nkb,stages", [(1, 2), (2, 2), (5, 3), (12, 4)])
+def test_gemm_ring_pipeline(nkb, stages):
+    for seed in range(60):
+        sim_gemm_ring(nkb, stages, seed)
+
+
+@pytest.mark.parametrize("nt", [1, 2, 5])
+def test_attention_forward_pipeline(nt):
+    for seed in range(60):
+        sim_attention(nt, ["Q"], ["K", "V"], [("Q", "K")], [("V", "O")], seed, ["O"])
+
+
 def test_the_simulator_catches_a_missing_wait():
-    """Self-check: a TMA producer that does NOT wait for the K/V slot to be released (kv_empty) refills K under MMAs that still
-    read it; the simulation must report that on some schedule.  (In this one-tile-in-flight design several other waits -- s_free,
-    ds_free -- are implied transitively by kv_empty; they are kept in the kernels as the pipeline is meant to be deepened.)"""
-    def broken(seed):
+    """Self-check: a warpgroup that releases the slot of block i right after issuing its MMAs (no wgmma_wait before the arrive)
+    lets the producer refill it under MMAs that still read it; the simulation must report that on some schedule."""
+    def broken(seed, stages=2, nkb=6):
         s = Sim(seed)
-        kv_full, s_full, ds_full = MBar(1), MBar(1), MBar(4)
-        s.mem.update({"K": None, "dS": None, "S": None, "dQ": ("dQ", -1)})
+        full, empty = [MBar(1) for _ in range(stages)], [MBar(1) for _ in range(stages)]
+        for st in range(stages):
+            s.mem[f"A{st}"] = None
+        s.mem["acc"] = ("acc", -1)
 
         def producer():
-            for j in range(4):                               # no kv_empty wait
-                kv_full.expect_tx(1)
-                s.tma("K", ("K", j), kv_full, 1)
-                yield wait(kv_full, j & 1)                   # (only waits for its own copy to land)
-
-        def mma():
-            for j in range(4):
-                yield wait(kv_full, j & 1)
-                s.mma([("K", ("K", j))], ("S", ("S", j)))
-                s.commit(s_full)
-                yield wait(ds_full, j & 1)
-                s.mma([("dS", ("dS", j)), ("K", ("K", j))], ("dQ", ("dQ", j)), chain=[("dQ", ("dQ", j - 1))])
+            for i in range(nkb):
+                st = i % stages
+                yield wait(empty[st], ((i // stages) & 1) ^ 1)
+                full[st].expect_tx(1)
+                s.tma(f"A{st}", ("A", i), full[st], 1)
                 yield None
 
-        def softmax(w):
-            def g():
-                for j in range(4):
-                    yield wait(s_full, j & 1)
-                    if w == 3:
-                        s.mem["dS"] = ("dS", j)
-                    yield None
-                    ds_full.arrive()
-            return g()
+        def mma():
+            for i in range(nkb):
+                st = i % stages
+                yield wait(full[st], (i // stages) & 1)
+                s.mma([(f"A{st}", ("A", i))], ("acc", ("acc", i)), chain=[("acc", ("acc", i - 1))])
+                s.group()
+                empty[st].arrive()                       # BUG: no wgmma_wait before the release
+                yield None
+            yield wgmma_wait(s, 0)
 
         s.spawn("tma", producer())
         s.spawn("mma", mma())
-        for w in range(4):
-            s.spawn(f"sm{w}", softmax(w))
         s.run()
 
     caught = 0

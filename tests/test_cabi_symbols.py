@@ -28,12 +28,12 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, s), f"{s} declared in include/chatts_b200.h but not exported"
     assert sorted(_cabi.SYMBOLS) == syms, "chatts_b200/_cabi.py SYMBOLS out of sync with the header"
     lib.cts_arch.restype = ctypes.c_char_p
-    assert lib.cts_arch() == b"sm_100a"
+    assert lib.cts_arch() == b"sm_90a"
     assert lib.cts_version() >= 100
 
 
-def test_sass_is_blackwell_native():
-    """tcgen05 / TMA must be in the shipped SASS (UTCHMMA, UTMALDG, LDTM: B200_PROFILING.md 'what proves...')."""
+def test_sass_is_hopper_native():
+    """wgmma / TMA must be in the shipped SASS (HGMMA, UTMALDG), next to the warp-level HMMA of the attention kernels."""
     import shutil
     import subprocess
     from chatts_b200 import _cabi
@@ -41,9 +41,9 @@ def test_sass_is_blackwell_native():
         pytest.skip("cuobjdump not available")
     exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     sass = subprocess.run([exe, "-sass", _cabi.LIB_PATH], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "HMMA"):
+    for mnemonic in ("HGMMA", "UTMALDG", "HMMA"):
         assert mnemonic in sass, mnemonic
-    assert "sm_100a" in subprocess.run([exe, "-lelf", _cabi.LIB_PATH], capture_output=True, text=True).stdout
+    assert "sm_90a" in subprocess.run([exe, "-lelf", _cabi.LIB_PATH], capture_output=True, text=True).stdout
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")

@@ -1,6 +1,6 @@
 """The LOGIC of the training / sampling / executor GPU tests (shapes, arguments, reference arithmetic, tolerances) is exercised on
 CPU on every run: tools/dryrun_train_gpu_tests.py executes those test files with the C-ABI replaced by the torch test double, in a
-subprocess (it monkeypatches torch.cuda).  A red B200 run of those files then points at a kernel, not at a test bug."""
+subprocess (it monkeypatches torch.cuda).  A red GPU run of those files then points at a kernel, not at a test bug."""
 import os
 import subprocess
 import sys

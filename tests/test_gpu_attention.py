@@ -25,18 +25,16 @@ def test_prefill_fp16(d):
 @pytest.mark.parametrize("DT", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("lens", [[577], [300, 129, 64]])
 def test_prefill_growing_scores_force_the_lazy_rescale(lens, DT):
-    """The tcgen05 kernel keeps a row's exponent maximum until a tile exceeds it by more than 8 (log2 units) and then rescales l and the
-    O accumulator in TMEM in place.  Random data rarely moves the maximum after the first tile; here the scores grow along the sequence
-    (keys scaled by their position), so every 64-key tile raises the maximum by far more than the threshold for most rows -- the rescale
-    path runs in nearly every tile, for some rows of a warp and not for others."""
+    """The wgmma kernel rescales l and the O accumulator registers whenever a tile raises a row's running maximum.  Random data
+    rarely moves the maximum after the first tile; here the scores grow along the sequence (keys scaled by their position), so every
+    64-key tile raises the maximum for most rows -- the rescale runs in nearly every tile, with large correction factors."""
     _prefill_case(128, lens, DT, ramp=True)
 
 
 @pytest.mark.parametrize("DT", [torch.bfloat16, torch.float16])
 def test_prefill_many_items_per_persistent_cta(DT):
-    """The tcgen05 kernel runs 2 x SMs persistent CTAs over the (query tile, head, sequence) items.  40 sequences x 8 heads x 3 query
-    tiles = 960 items: every CTA walks through three or four of them -- dead ones (sequences shorter than the longest) included -- so the
-    barrier phases, the Q hand-over (q_free) and the O hand-over (o_free) carry across items."""
+    """40 sequences x 8 heads x 3 query tiles = 960 (query tile, head, sequence) items, many of them dead (sequences shorter than the
+    longest): the wgmma kernel's grid covers every item, and the CTAs of dead items must leave before issuing anything."""
     lens = [300, 17, 129, 256, 1, 64, 200, 299, 128, 65] * 4
     _prefill_case(128, lens, DT, nh=8)
 

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM through the C-ABI against fp32 torch on the CPU (same bf16/fp16 inputs)."""
+"""wgmma GEMM through the C-ABI against fp32 torch on the CPU (same bf16/fp16 inputs)."""
 import pytest
 import torch
 

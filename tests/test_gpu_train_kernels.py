@@ -1,5 +1,4 @@
-"""sm_100a kernels of the LoRA fine-tune step (row A9) that HAVE run on a B200 (profiles/r1_train_kernels_first_b200_run.log,
-29 passed on their first execution): the small-N / small-K LoRA GEMM shapes, SwiGLU forward/backward, RMSNorm backward,
+"""Kernels of the LoRA fine-tune step (row A9): the small-N / small-K LoRA GEMM shapes, SwiGLU forward/backward, RMSNorm backward,
 RoPE(+q/k-norm) backward, fused cross entropy, row gather and the LoRA weight-gradient kernel -- through the C-ABI against
 the torch restatement of every entry point (tests/cabi_double.py, fp32 on the CPU, itself checked against oracle/lora.py by
 tests/test_host_train.py).  The parts of the training path still waiting for their first GPU run live in

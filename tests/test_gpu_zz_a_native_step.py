@@ -1,6 +1,6 @@
 """cts_decoder_step / cts_rmsnorm / cts_lm_head (csrc/decoder_step.cu: host-side executors over the validated kernels) against
 the per-kernel Python orchestration: the same launches in the same order must give bit-identical tokens and logits.
-First executed on a B200 by the round-1 driver run (GPUTEST_r01.json); plain tests since round 2 (no xfail markers)."""
+Plain tests (no xfail markers)."""
 import numpy as np
 import pytest
 import torch

@@ -1,6 +1,5 @@
 """cts_sample_advance (csrc/sampling.cu) against its CPU statement (tests/cabi_double.py ``sample_reference``, itself checked
-against transformers' logits warpers in tests/test_host_sampling.py).  Validated on a B200 by the round-1
-driver run (GPUTEST_r01.json: every case passed); plain tests since round 2."""
+against transformers' logits warpers in tests/test_host_sampling.py)."""
 import numpy as np
 import pytest
 import torch

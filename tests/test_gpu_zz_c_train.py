@@ -1,8 +1,6 @@
 """The part of the LoRA fine-tune step (row A9) that was written after the round-1 GPU budget was spent: the attention LSE flag, the attention
-backward (HMMA), AdamW + clip, adapter packing and the whole-step tests against oracle/lora.py -- compiled for sm_100a,
-orchestration parity-checked on CPU through the double (tools/dryrun_train_gpu_tests.py runs this file's logic on CPU), written
-after the round-1 GPU budget was spent and validated by the round-1 driver run on a B200 (every case passed); plain tests
-since round 2.  The kernels validated earlier are in tests/test_gpu_train_kernels.py.  The zz files
+backward (HMMA), AdamW + clip, adapter packing and the whole-step tests against oracle/lora.py -- compiled for sm_90a,
+orchestration parity-checked on CPU through the double (tools/dryrun_train_gpu_tests.py runs this file's logic on CPU).  The kernels validated earlier are in tests/test_gpu_train_kernels.py.  The zz files
 sort last on purpose (a sticky CUDA error here cannot poison validated tests); none of the kernels exercised here spins on a
 flag."""
 import math

@@ -5,7 +5,7 @@ does over NVLink, minus the link.  The W kernels of a call spin on each other an
 W x C x T <= 128 CTAs of 256 threads (one per SM suffices), and the kernel's bounded polls turn a scheduling surprise into a trap
 instead of a hang.  Expected values: the rank-ordered fp32 sum formed step by step (bit-exact h), RMSNorm from h (tolerance: the
 statistic's summation order differs from torch's), bit-identical results on all ranks.
-Validated on a B200 by the round-1 driver run (every case passed); plain tests since round 2.  The protocol
+The protocol
 itself is model-checked on CPU in tests/test_peer_ll_protocol.py."""
 import pytest
 import torch

@@ -53,7 +53,7 @@ def test_gptq_checkpoint_decodes_through_the_packed_weights(cabi_double, tmp_pat
     from chatts_b200.model import ChatTSForCausalLM
     monkeypatch.setenv("CTS_W4_KERNEL", kernel)
     cfg, sd, _, proc = _build(cabi_double)
-    if kernel == "mma":          # the mma kernel's pipeline stage is 128 K wide: the tiny config's 704-wide MLP (5.5 x 128) is for the tcgen05 kernel
+    if kernel == "mma":          # the mma kernel's pipeline stage is 128 K wide: the tiny config's 704-wide MLP (5.5 x 128) is for the wgmma kernel
         from chatts_b200.weights import synthetic_state_dict
         cfg.intermediate_size = 768
         sd = synthetic_state_dict(cfg, seed=1234, device="cpu", dtype=torch.bfloat16, std=0.05)

@@ -3,9 +3,9 @@
 product's own ctypes wrappers drive them on host memory:
 
   * tools/shim_gpu_tests.py runs the GPU test cases of the sampling kernel, AdamW + clip, adapter packing, the attention backward
-    (attention_bwd.cu: wmma through a fragment shim) and -- in a HYBRID context where the tcgen05 GEMMs and the attention forward are
-    answered by the torch double -- the whole LoRA training step against the oracle (all still pending on a B200), plus, as
-    calibration of the shim itself, the elementwise / cross-entropy / weight-gradient tests that already passed on a B200
+    (attention_bwd.cu: wmma through a fragment shim) and -- in a HYBRID context where the wgmma GEMMs and the attention forward are
+    answered by the torch double -- the whole LoRA training step against the oracle, plus, as
+    calibration of the shim itself, the elementwise / cross-entropy / weight-gradient tests that pass on the GPU
     (the CPU suite runs the --quick subset; the full selection is 56 cases in about 4 minutes);
   * the low-latency all-reduce (allreduce_ll.cu) runs with its ranks as PROCESSES sharing the symmetric regions: real concurrency
     between ranks, torn 16-byte units, consecutive calls without any barrier in between.
@@ -30,8 +30,8 @@ def test_pending_and_validated_kernels_pass_their_gpu_tests_on_the_shim():
     assert r.returncode == 0, tail
     import re
     passed = [int(n) for n in re.findall(r"(\d+) passed", r.stdout)]
-    # sampling, training (incl. one whole step), validated elementwise kernels, cluster-fused decode GEMMs, validated GEMMs, tcgen05 backward,
-    # single-pass persistent prefill attention, W4A16 mma GEMM
+    # sampling, training (incl. one whole step), validated elementwise kernels, cluster-fused decode GEMMs, validated GEMMs, wgmma
+    # attention backward, prefill attention, W4A16 mma GEMM
     assert len(passed) == 8 and min(passed) >= 1 and sum(passed) >= 118 and "failed" not in r.stdout, tail
     native = r.stdout.split("entry points running from kernel source:")[1].split("\n")[0].split()
     assert {"sample_advance", "attn_bwd", "adamw", "grad_norm_clip", "lora_pack", "lora_wgrad", "ce_loss_grad", "rmsnorm_bwd", "swiglu_bwd",
@@ -105,7 +105,7 @@ def test_ll_allreduce_kernel_with_ranks_as_processes(W, T, h, split, dt):
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-# gemm_decode_fused.cu through the shim: the TMA -> tcgen05 -> TMEM mainloop is replaced (inside the kernel, #ifdef CTS_HOST_SHIM) by
+# gemm_decode_fused.cu through the shim: the TMA -> wgmma mainloop is replaced (inside the kernel, #ifdef CTS_HOST_SHIM) by
 # the fp32 partial tile it produces; from the cluster barrier on the kernel runs AS WRITTEN: the K splits of a tile as the CTAs of
 # one cluster (threads here), the distributed-shared-memory reduction in split order, the three tails, the fused RMSNorm operand,
 # and the in-kernel all-reduce with ranks as processes.  Reference: the torch double's statement of the two-launch path.  The
@@ -252,7 +252,7 @@ def test_fused_gemm_allreduce_tail_with_ranks_as_processes(shim_ctx, W, T, N, Kr
     assert [int(s_[0]) for s_ in state] == [len(calls)] * W
 
 
-# the all-reduce-inside-the-GEMM variant is an opt-in path that measured slower on the B200 (DESIGN.md section 5): it runs here only with
+# the all-reduce-inside-the-GEMM variant is an opt-in path: it runs here only with
 # CTS_SLOW_TESTS=1, to keep the default CPU suite within a few minutes on a busy machine
 _TP_VARIANTS = ["CTS_PEER_LL=1"] + (["CTS_PEER_LL=1 CTS_DECODE_FUSED=2"] if os.environ.get("CTS_SLOW_TESTS") == "1" else [])
 
@@ -277,7 +277,7 @@ def test_tensor_parallel_model_with_ranks_as_processes(variant):
     assert "identical tokens on all ranks: True" in out and "greedy agreement [8, 8]/8" in out, out[-2000:]
 
 
-@pytest.mark.skipif(os.environ.get("CTS_SLOW_TESTS") != "1", reason="the guard of bench.py's opt-in --probe (decode variants that measured slower on the B200); CTS_SLOW_TESTS=1 runs it")
+@pytest.mark.skipif(os.environ.get("CTS_SLOW_TESTS") != "1", reason="the guard of bench.py's opt-in --probe (opt-in decode variants, off by default); CTS_SLOW_TESTS=1 runs it")
 def test_numeric_guard_of_the_decode_variant_probe_runs_from_source():
     """tools/probe_decode_variant.py (the child bench.py runs before it adopts fusion level 2): default path and variant on the same weights,
     teacher-forced, logits compared at every step -- executed here through the shim with a toy configuration."""

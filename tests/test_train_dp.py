@@ -1,4 +1,4 @@
-"""Data-parallel LoRA step on CPU with two real processes over gloo (config 5 is 4 x B200 data parallel): every rank runs
+"""Data-parallel LoRA step on CPU with two real processes over gloo (config 5 is 4-GPU data parallel): every rank runs
 LoraTrainer through the torch test double on ITS shard of the records; one all-reduce of the gradient arena must give the
 step a single process computes on the union of the records (token-mean over the global batch)."""
 import os

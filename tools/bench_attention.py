@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The tcgen05 prefill attention kernel ALONE (no model): causal-useful TFLOP/s at the benchmark shape (32 x 576, 40 / 8 heads of 128)
+"""The wgmma prefill attention kernel ALONE (no model): causal-useful TFLOP/s at the benchmark shape (32 x 576, 40 / 8 heads of 128)
 and at two longer ones, next to the attention kernels installed on the box (library code, a stated comparison only).  One JSON line.
 `--once` runs the benchmark shape a few times only (for ncu)."""
 import json

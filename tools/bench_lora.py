@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench_lora.py -- BASELINE config 5: ChatTS-8B LoRA fine-tune step (forward + backward + clip + AdamW) on N B200s,
+"""bench_lora.py -- BASELINE config 5: ChatTS-8B LoRA fine-tune step (forward + backward + clip + AdamW) on N GPUs,
 data parallel.  Same measurement contract as bench.py (one JSON line on rank 0; CUDA events; barrier + synchronize on
 both sides; max over ranks; clocks sampled during the timed region), for the SECOND workload of the hot path -- bench.py
 itself stays on the headline decode metric.
@@ -57,7 +57,7 @@ def tensor_peak():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "measured (MEASURED_PEAKS.json, sustained cuBLAS bf16)"
-    return 1440.0, "fallback (B200_PROFILING.md)"
+    return 989.0, "H100 SXM data sheet (dense bf16)"
 
 
 def step_flops(cfg, positions, label_rows, lens):

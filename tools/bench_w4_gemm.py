@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """The two W4A16 decode GEMMs alone at the ChatTS-14B projection shapes: packed GB/s per launch (distinct weights per launch, >> L2)
 for several split factors and token counts, next to the bf16 decode GEMM on the dequantised weight.
-   cts_gemm_w4      (tcgen05 operand path, csrc/gemm_w4.cu)      -- T = 32 only (the round's earlier records)
+   cts_gemm_w4      (wgmma operand path, csrc/gemm_w4.cu)        -- T = 32 only
    cts_gemm_w4_mma  (registers + mma.sync, csrc/gemm_w4_mma.cu) -- T = 1 / 8 / 16 / 32
-`--once` runs a few launches of the mma kernel only (for ncu); W4_TC5=0 skips the tcgen05 kernel."""
+`--once` runs a few launches of the mma kernel only (for ncu); W4_TC5=0 skips the wgmma kernel."""
 import json, os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Dry run of the benchmark drivers on a machine WITHOUT a GPU (TEST INFRASTRUCTURE ONLY -- not a measurement).
 
-    python tools/dryrun_bench.py decode      # bench.py's B200 arm
+    python tools/dryrun_bench.py decode      # bench.py's native arm
     python tools/dryrun_bench.py lora        # tools/bench_lora.py
 
 The C-ABI is replaced by the torch test double (tests/cabi_double.py), `device="cuda"` is dropped, CUDA events / graphs / clock

@@ -1,6 +1,6 @@
 """Dry-run of the training / sampling / native-step GPU test files on a machine WITHOUT a GPU: `ctx()` returns the torch test double, `.cuda()` is the
 identity and `device="cuda"` is dropped, so the TEST LOGIC (shapes, arguments, reference arithmetic, tolerances) is
-exercised end to end.  A failure on the B200 then points at a kernel, not at the test.  TEST INFRASTRUCTURE ONLY.
+exercised end to end.  A failure on the GPU then points at a kernel, not at the test.  TEST INFRASTRUCTURE ONLY.
 
     python tools/dryrun_train_gpu_tests.py [pytest args]
 """
@@ -47,5 +47,5 @@ extra = sys.argv[1:]
 if "-k" not in extra:          # the ChatTS-8B-shaped case generates its weights on the device: GPU only
     extra += ["-k", "not (directional and True)"]
 sys.exit(pytest.main([os.path.join(ROOT, "tests", f) for f in ("test_gpu_train_kernels.py", "test_gpu_zz_c_train.py", "test_gpu_zz_b_sampling.py", "test_gpu_zz_a_native_step.py",
-                                                         "test_gpu_zz_d_attn_bwd_tc5.py", "test_gpu_zz_e_fused_decode.py")] +
+                                                         "test_gpu_zz_d_attn_bwd_wgmma.py", "test_gpu_zz_e_fused_decode.py")] +
                      ["-q", "-p", "no:cacheprovider", "--runxfail", "-m", "gpu"] + extra))

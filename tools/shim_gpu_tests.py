@@ -1,6 +1,6 @@
 """GPU tests executed on a machine WITHOUT a GPU through the "CUDA on CPU" shim (tests/cuda_on_cpu): `ctx()` returns a Context whose library
 is the kernels' own source compiled by g++ -- CUDA threads as fibers, clusters as threads, and a functional emulation of mbarrier / TMA /
-TMEM / tcgen05.mma that is calibrated by the GPU-validated GEMM kernels passing their own test file -- and `.cuda()` is the identity.
+wgmma that is calibrated by the GPU-validated GEMM kernels passing their own test file -- and `.cuda()` is the identity.
 Unlike tools/dryrun_train_gpu_tests.py (which checks the TEST LOGIC against the torch double), this executes the KERNEL SOURCE.
 TEST INFRASTRUCTURE ONLY.
 
@@ -65,7 +65,7 @@ import tests.gpu_util as gu  # noqa: E402
 _ctx = shim_context()
 from tests.cabi_double import TorchDouble as _TD  # noqa: E402
 _dbl = _TD()
-# HYBRID context for the whole-step tests: every entry point whose source is in the shim build runs that source; the others (tcgen05
+# HYBRID context for the whole-step tests: every entry point whose source is in the shim build runs that source; the others (wgmma
 # GEMMs, attention forward, the decode-side kernels) are answered by the torch double.  What this adds over the double-only dry run:
 # train.py's argument plumbing (strides, interleaved layouts, arena offsets, packing descriptors) meets the REAL backward / loss /
 # optimiser kernels.
@@ -102,17 +102,17 @@ SELECT = {
     "test_gpu_zz_b_sampling.py": None,
     "test_gpu_zz_c_train.py": "adamw_and_clip or lora_pack or prefill_lse or test_attention_backward or train_step_matches_oracle or training_reduces_loss or (directional and False) or wgrad_tensor_core",
     "test_gpu_train_kernels.py": None,
-    # the cluster-fused decode GEMMs against the two-launch path, BIT FOR BIT: both GEMM kernels run from source through the tcgen05 /
+    # the cluster-fused decode GEMMs against the two-launch path, BIT FOR BIT: both GEMM kernels run from source through the wgmma /
     # TMA / mbarrier emulation of the shim (same accumulation order), the reduce kernels of the two-launch path come from the double
     "test_gpu_zz_e_fused_decode.py": None,
     "test_gpu_gemm.py": None,                            # calibration of the emulation: the GPU-validated GEMM kernels themselves
     "test_gpu_elementwise.py": None,                     # calibration: split-K tails, RoPE / KV write, RMSNorm over a cluster (DSMEM), argmax + advance
     "test_gpu_ts_encoder.py": None,                      # calibration: the TS encoder against the reference-generated fixtures
-    "test_gpu_zz_a_native_step.py": None,                # cts_decoder_step / cts_ts_encode: the C++ executors over the kernels above (pending on a B200)
+    "test_gpu_zz_a_native_step.py": None,                # cts_decoder_step / cts_ts_encode: the C++ executors over the kernels above 
     "test_gpu_model.py": "not full_size",                # calibration: the whole model (prefill, paged decode, generate, LoRA merge ...) from kernel source
-    "test_gpu_attention.py": None,                       # calibration: tcgen05 prefill attention (MN-major V operand), HMMA prefill, TMA paged decode (ldmatrix / mma.sync)
-    "test_gpu_zz_d_attn_bwd_tc5.py": None,               # tcgen05 attention backward (K-major and MN-major operands, TMEM-resident dQ / dK / dV)
-    "test_gpu_w4.py": "not (27648 or 13824 or 7168)",    # both W4A16 kernels (tcgen05 operand path; registers + mma.sync over the persistent schedule), small shapes
+    "test_gpu_attention.py": None,                       # calibration: HMMA prefill, TMA paged decode (ldmatrix / mma.sync)
+    "test_gpu_zz_d_attn_bwd_wgmma.py": None,             # wgmma attention backward (K-major and MN-major operands, register-A MMAs)
+    "test_gpu_w4.py": "not (27648 or 13824 or 7168)",    # both W4A16 kernels (wgmma operand path; registers + mma.sync over the persistent schedule), small shapes
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
@@ -122,9 +122,8 @@ QUICK = {
     "test_gpu_train_kernels.py": None,
     "test_gpu_zz_e_fused_decode.py": None,
     "test_gpu_gemm.py": "not deterministic_under_repetition",
-    "test_gpu_zz_d_attn_bwd_tc5.py": "lens0 or lens1 or lens4",
-    # the two kernels of round 2's second session: the persistent single-pass prefill attention (the lazy-rescale and the many-items cases)
-    # and the W4A16 mma kernel (two small shapes, both dtypes)
+    "test_gpu_zz_d_attn_bwd_wgmma.py": "lens0 or lens1",
+    # the prefill attention (the growing-maximum and the many-items cases) and the W4A16 mma kernel (two small shapes, both dtypes)
     "test_gpu_attention.py": "growing or many_items",
     "test_gpu_w4.py": "mma_partials and (256-512-128-5-2 or 528-1536)",
 }

@@ -4,7 +4,7 @@ cold, so it cannot show where the HBM stream idles between the ~440 PDL-chained 
 device-side trace buffer, replays the captured step once, and writes the raw {tag, %globaltimer} records
 (gpurun_out/trace_b<B>.npy) plus a per-launch table; `--analyze file.npy` re-runs the analysis offline.
 
-    python tools/trace_decode_step.py --batch 32 [--layers N]        # on the B200
+    python tools/trace_decode_step.py --batch 32 [--layers N]        # on the GPU
     python tools/trace_decode_step.py --analyze gpurun_out/trace_b32.npy
 
 The traced replay is a diagnostic run (atomics + timer reads in every CTA): none of its times is a benchmark value."""
