@@ -31,6 +31,7 @@ SYMBOLS = [
     "cts_sample_advance", "cts_rmsnorm", "cts_lm_head", "cts_decoder_step_ws_floats", "cts_decoder_step", "cts_ts_encode", "cts_gemm_decode_fused",
     "cts_peer_ll_region_bytes", "cts_peer_allreduce_ll", "cts_trace_enable", "cts_ts_encode_fused_ok", "cts_ts_encode_fused",
     "cts_rep_penalty_mark", "cts_rep_penalty_apply", "cts_gemm_w4", "cts_gemm_w4_suggest_split", "cts_gemm_w4_mma", "cts_gemm_w4_mma_suggest_split",
+    "cts_gemm_fp8", "cts_gemm_fp8_suggest_split", "cts_fp8_dequant",
 ]
 FUSED_RESIDUAL, FUSED_SWIGLU, FUSED_QKV_ROPE = 0, 1, 2
 PACK_DESC_LONGS = 12
@@ -101,6 +102,17 @@ class GemmW4fArgs(C.Structure):
                 ("group_size", C.c_int), ("split_k", C.c_int), ("dtype", C.c_int), ("reserved", C.c_int)]
 
 
+class GemmFp8Args(C.Structure):
+    _fields_ = [("qw", C.c_void_p), ("scales", C.c_void_p), ("x", C.c_void_p), ("out", C.c_void_p),
+                ("n", C.c_longlong), ("k", C.c_longlong), ("t", C.c_longlong), ("x_ld", C.c_longlong),
+                ("split_k", C.c_int), ("dtype", C.c_int), ("reserved0", C.c_int), ("reserved1", C.c_int)]
+
+
+class Fp8DequantArgs(C.Structure):
+    _fields_ = [("qw", C.c_void_p), ("scales", C.c_void_p), ("out", C.c_void_p),
+                ("n", C.c_longlong), ("k", C.c_longlong), ("out_ld", C.c_longlong), ("dtype", C.c_int), ("reserved", C.c_int)]
+
+
 class TsEncodeArgs(C.Structure):
     _fields_ = ([("x", C.c_void_p)] + [(k, C.c_int) for k in ("dtype", "n_series", "row_len", "num_features", "patch_size", "mode")] +
                 [("pos_table", C.c_void_p)] + [(k, C.c_int) for k in ("emb_dim", "max_seq_len", "num_layers", "hidden", "in0")] +
@@ -158,6 +170,9 @@ def load_library():
     lib.cts_gemm_w4_suggest_split.argtypes = [vp, ll, ll]
     lib.cts_gemm_w4_mma.argtypes = [vp, C.POINTER(GemmW4fArgs), vp]
     lib.cts_gemm_w4_mma_suggest_split.argtypes = [vp, ll, ll, ll]
+    lib.cts_gemm_fp8.argtypes = [vp, C.POINTER(GemmFp8Args), vp]
+    lib.cts_gemm_fp8_suggest_split.argtypes = [vp, ll, ll, ll]
+    lib.cts_fp8_dequant.argtypes = [vp, C.POINTER(Fp8DequantArgs), vp]
     lib.cts_rep_penalty_mark.argtypes = [vp, vp, vp, i, vp, i, ll, vp]
     lib.cts_rep_penalty_apply.argtypes = [vp, vp, ll, ll, i, vp, i, f, i, vp]
     lib.cts_ts_encode_fused_ok.argtypes = [C.POINTER(TsEncodeArgs)]
@@ -349,6 +364,26 @@ class Context:
 
     def gemm_w4_mma_suggest_split(self, n, k, t=1):
         return int(self.lib.cts_gemm_w4_mma_suggest_split(self.h, n, k, t))
+
+    def gemm_fp8(self, x, qw, scales, k, out, split_k, t=None):
+        """fp32 split-K partials [S, T, N] of x[T, K] @ W^T for FP8 weights, W[n] = scales[n] * e4m3(codes[n]) (cts_gemm_fp8; decode-sized
+        T).  qw uint8 [ceil(N/256) * K/64 * 16384] fragment-major codes (weights.py:pack_fp8_mma), scales fp32 [N]."""
+        a = GemmFp8Args()
+        a.qw, a.scales, a.x, a.out = qw.data_ptr(), scales.data_ptr(), x.data_ptr(), out.data_ptr()
+        a.n, a.k = scales.shape[0], int(k)
+        a.t = x.shape[0] if t is None else t
+        a.x_ld, a.split_k, a.dtype = x.stride(0), int(split_k), dtype_code(x.dtype)
+        self._chk(self.lib.cts_gemm_fp8(self.h, C.byref(a), _stream()))
+
+    def gemm_fp8_suggest_split(self, n, k, t=1):
+        return int(self.lib.cts_gemm_fp8_suggest_split(self.h, n, k, t))
+
+    def fp8_dequant(self, qw, scales, k, out):
+        """out[:N, :K] = dtype(fp32(e4m3(codes)) * scales[:, None]) from the layout of gemm_fp8 (cts_fp8_dequant); out [>= N, K] 16-bit."""
+        a = Fp8DequantArgs()
+        a.qw, a.scales, a.out = qw.data_ptr(), scales.data_ptr(), out.data_ptr()
+        a.n, a.k, a.out_ld, a.dtype = scales.shape[0], int(k), out.stride(0), dtype_code(out.dtype)
+        self._chk(self.lib.cts_fp8_dequant(self.h, C.byref(a), _stream()), 2)
 
     # ------------------------------------------------------------------ fused split-K tails
     def reduce_bias_act(self, partial, split_k, t, n, bias, act, out, row_map=None):

@@ -57,6 +57,11 @@ class PagePool:
         self.free.extend(reversed(pages))
 
 
+def _check_quantization(quantization):
+    if quantization not in (None, "fp8"):
+        raise ValueError(f"quantization={quantization!r}: supported are None (the checkpoint's 16-bit weights) and 'fp8'")
+
+
 class _Step:
     """Static buffers of one decode configuration (batch size) + its captured CUDA graphs."""
     pass
@@ -114,6 +119,7 @@ class ChatTSForCausalLM:
         # prefetched lines do not survive the current GEMM's stream through L2, so the bytes are read twice.  CTS_NEXT_PREFETCH_MB=<n> turns it on for experiments.
         self.next_prefetch_bytes = int(float(_os.environ.get("CTS_NEXT_PREFETCH_MB", "0")) * (1 << 20))
         self.w4 = None               # W4A16 decode weights (csrc/gemm_w4.cu): set by attach_w4 / quantize_w4_synthetic / from_pretrained(GPTQ)
+        self.fp8 = None              # FP8 projection weights (csrc/gemm_fp8.cu): set by quantize_fp8
         self._load(state_dict)
         # every position the page table can address has a row in the rotary tables (max_pages * page_size >= max_seq_len), capped by
         # the model's max_position_embeddings; _alloc_pages rejects sequences beyond it (no silent out-of-bounds cos/sin read)
@@ -169,16 +175,21 @@ class ChatTSForCausalLM:
         self.ts_encoder = TimeSeriesEmbedding(cfg.ts, ts_w, device=dev, dtype=dt) if ts_w else None
 
     @classmethod
-    def from_synthetic(cls, config=None, seed=1234, device="cuda", dtype=torch.bfloat16, gen_device=None, **kw):
+    def from_synthetic(cls, config=None, seed=1234, device="cuda", dtype=torch.bfloat16, gen_device=None, quantization=None, **kw):
         """Random-init weights at the config's shapes (no checkpoint exists offline).  ``gen_device='cpu'`` gives
-        values identical to the CPU oracle's; the default generates on the GPU (14B in seconds)."""
+        values identical to the CPU oracle's; the default generates on the GPU (14B in seconds).  quantization="fp8": quantize_fp8()."""
+        _check_quantization(quantization)
         config = config or ChatTSConfig.chatts_14b()
         sd = synthetic_state_dict(config, seed=seed, device=gen_device or device, dtype=dtype)
-        return cls(config, sd, device=device, dtype=dtype, **kw)
+        model = cls(config, sd, device=device, dtype=dtype, **kw)
+        del sd
+        return model.quantize_fp8() if quantization == "fp8" else model
 
     @classmethod
-    def from_pretrained(cls, path, device_map=None, torch_dtype=None, trust_remote_code=True, device=None, **kw):
-        """AutoModelForCausalLM.from_pretrained surface (README.md:88): config.json + safetensors shards."""
+    def from_pretrained(cls, path, device_map=None, torch_dtype=None, trust_remote_code=True, device=None, quantization=None, **kw):
+        """AutoModelForCausalLM.from_pretrained surface (README.md:88): config.json + safetensors shards.  quantization="fp8": the
+        decoder projections are quantised to FP8 at load time (quantize_fp8); None keeps the checkpoint's dtype."""
+        _check_quantization(quantization)
         cfg = ChatTSConfig.from_json(path)
         dt = {"float16": torch.float16, "bfloat16": torch.bfloat16, torch.float16: torch.float16,
               torch.bfloat16: torch.bfloat16, None: getattr(torch, cfg.torch_dtype, torch.bfloat16)}[torch_dtype]
@@ -186,6 +197,8 @@ class ChatTSForCausalLM:
         sd = load_checkpoint(path, device="cpu")
         w4_packed, w4_gs = None, 0
         if any(k.endswith(".qweight") for k in sd):                # GPTQ-Int4 checkpoint (README.md:52,262-263)
+            if quantization is not None:
+                raise ValueError(f"quantization={quantization!r} applies to 16-bit checkpoints; {path} is already GPTQ-quantised")
             import json as _json
             import os as _os
             from .weights import dequantize_gptq, gptq_w4_pack
@@ -198,8 +211,11 @@ class ChatTSForCausalLM:
                 w4_packed, w4_gs = gptq_w4_pack(sd, qc, dtype=dt)
             sd = dequantize_gptq(sd, qc, dtype=dt, scale_dtype=dt if w4_packed is not None else None)
         model = cls(cfg, sd, device=dev, dtype=dt, **kw)
+        del sd
         if w4_packed is not None:
             model.attach_w4(w4_packed, w4_gs)
+        if quantization == "fp8":
+            model.quantize_fp8()
         # generation_config.json: the defaults HF's generate() applies when the caller passes none (README.md:102 calls
         # model.generate(**inputs, max_new_tokens=300) with no sampling arguments)
         import json as _json2
@@ -221,6 +237,9 @@ class ChatTSForCausalLM:
         import json
         import os
         import re
+        if self.fp8 is not None:
+            raise ValueError("merge_lora on an FP8 model: the 16-bit projection weights are gone -- merge the adapter into the 16-bit "
+                             "model first, then call quantize_fp8()")
         if isinstance(adapter, str):
             cfg_path = os.path.join(adapter, "adapter_config.json")
             if os.path.exists(cfg_path):
@@ -280,6 +299,8 @@ class ChatTSForCausalLM:
         values, i.e. weights.py:dequantize_gptq(..., scale_dtype=model dtype) -- HBM keeps both copies.  Fused operands
         are assembled exactly like the dense ones: q|k|v stacked, gate/up interleaved per 64 rows.  Single GPU (a tensor-parallel
         row split would cut groups: down_proj's 13824 / 8 = 1728 inputs are not a multiple of the group size)."""
+        if self.fp8 is not None:
+            raise ValueError("attach_w4 on an FP8 model: the projections are already quantised")
         if self.tp_size != 1:
             raise ValueError("W4A16 decode weights are single-GPU (tensor parallelism uses the dequantised weights)")
         dev = self.device
@@ -318,7 +339,7 @@ class ChatTSForCausalLM:
                     w4[kind][l] = repack_w4_mma(qw, sc, zp, gs) + (int(qw.shape[0]),)
             w4["splits"] = None           # per batch size: _w4_splits
         else:
-            w4["splits"] = dict(qkv=c.gemm_w4_suggest_split(self.wqkv[0].shape[0], self.H), o=c.gemm_w4_suggest_split(self.H, self.nh * self.d),
+            w4["splits"] = dict(qkv=c.gemm_w4_suggest_split(self._n_qkv, self.H), o=c.gemm_w4_suggest_split(self.H, self.nh * self.d),
                                 gu=c.gemm_w4_suggest_split(2 * self.I, self.H), d=c.gemm_w4_suggest_split(self.H, self.I))
         self.w4 = w4
         self._steps = {}                  # decode states (workspaces, captured graphs) are rebuilt for the new launches
@@ -329,6 +350,8 @@ class ChatTSForCausalLM:
         shapes, REPLACE the dense weights by their dequantised values and attach the packed copy -- a W4A16 model whose prefill and
         decode paths see the same weights."""
         from .weights import dequantize_w4, W4_NIBBLE_OF_K  # noqa: F401
+        if self.fp8 is not None:
+            raise ValueError("quantize_w4_synthetic on an FP8 model: the projections are already quantised")
         g = torch.Generator(device=self.device).manual_seed(seed)
         packed = {}
 
@@ -355,6 +378,70 @@ class ChatTSForCausalLM:
             del parts
         return self.attach_w4(packed, group_size)
 
+    # ------------------------------------------------------------------------------------------ FP8 weights (vLLM's quantization="fp8")
+    def quantize_fp8(self):
+        """Quantise the seven projections of every layer (fused q|k|v, gate/up interleaved, o, down) to FP8 in place: e4m3 codes (round
+        to nearest even) with one fp32 scale per output feature, s_n = max|W[n, :]| / 448 over the full checkpoint row (under tensor
+        parallelism the K-sliced o_proj / down_proj rows take the maximum over the ranks, so every rank holds a slice of the single-GPU
+        codes).  The 16-bit projection tensors are freed; embeddings, norms, biases, lm_head, the TS encoder and the KV cache stay in the
+        model dtype.  Decode-sized steps stream the codes (cts_gemm_fp8); every other step dequantises each projection into one
+        scratch matrix just before its GEMM (cts_fp8_dequant + cts_gemm).  Returns the model."""
+        from .weights import pack_fp8_mma, quantize_fp8_rows
+        if self.fp8 is not None:
+            raise ValueError("quantize_fp8() was already called on this model")
+        if self.w4 is not None:
+            raise ValueError("quantize_fp8 on a W4A16 model: its projections are already quantised")
+        kinds = (("qkv", self.wqkv, False), ("o", self.wo, True), ("gu", self.wgu, False), ("d", self.wd, True))
+        names = dict(qkv="self_attn.{q,k,v}_proj", o="self_attn.o_proj", gu="mlp.{gate,up}_proj", d="mlp.down_proj")
+        # every refusal before the first tensor is freed
+        for kind, ws, _ in kinds:
+            if ws[0].shape[1] % 64 != 0:
+                raise ValueError(f"quantize_fp8: {names[kind]} has {ws[0].shape[1]} input features per rank; the FP8 kernels need a multiple of 64")
+        for l in range(self.L):
+            for kind, ws, _ in kinds:
+                if not bool(torch.isfinite(ws[l]).all()):
+                    raise ValueError(f"quantize_fp8: model.layers.{l}.{names[kind]}.weight holds non-finite values")
+        fp8 = dict(qkv=[], o=[], gu=[], d=[])
+        biggest = 0
+        for l in range(self.L):
+            for kind, ws, row_parallel in kinds:
+                w = ws[l]
+                row_max = w.abs().amax(1).to(torch.float32)
+                if row_parallel and self.tp_size > 1:
+                    torch.distributed.all_reduce(row_max, op=torch.distributed.ReduceOp.MAX, group=self.comm)
+                codes, scales = quantize_fp8_rows(w, row_max, f"model.layers.{l}.{names[kind]}.weight")
+                fp8[kind].append((pack_fp8_mma(codes), scales, int(w.shape[1])))
+                biggest = max(biggest, w.numel())
+                ws[l] = None
+                del w, codes
+        # one scratch matrix for the dequantised projection of prefill-sized steps (stream order: each GEMM reads it before the next
+        # dequantisation overwrites it)
+        fp8["scratch"] = torch.empty(biggest, device=self.device, dtype=self.dtype)
+        self.fp8 = fp8
+        self._steps = {}
+        if hasattr(self, "_layer_list"):
+            del self._layer_list
+        if self.device.type == "cuda":
+            torch.cuda.empty_cache()
+        return self
+
+    def _fp8_dense(self, ent):
+        """16-bit row-major copy of one FP8 projection in the scratch matrix (prefill-sized steps)."""
+        qw, sc, k = ent
+        out = self.fp8["scratch"][: sc.shape[0] * k].view(sc.shape[0], k)
+        self.ctx.fp8_dequant(qw, sc, k, out)
+        return out
+
+    def _fp8_splits(self, T):
+        """Split-K factors of the four projections for an FP8 decode step of T tokens."""
+        c = self.ctx
+        return dict(qkv=c.gemm_fp8_suggest_split(self._n_qkv, self.H, T), o=c.gemm_fp8_suggest_split(self.H, self.nh * self.d, T),
+                    gu=c.gemm_fp8_suggest_split(2 * self.I, self.H, T), d=c.gemm_fp8_suggest_split(self.H, self.I, T))
+
+    @property
+    def _n_qkv(self):
+        return (self.nh + 2 * self.nkv) * self.d
+
     # ------------------------------------------------------------------------------------------ layers
     def _splits(self, T):
         c = self.ctx
@@ -363,11 +450,11 @@ class ChatTSForCausalLM:
         if ov and T <= 32:
             a = [int(v) for v in ov.split(",")]
             return dict(qkv=a[0], o=a[1], gu=a[2], d=a[3])
-        return dict(qkv=c.suggest_split(self.wqkv[0].shape[0], self.H, T), o=c.suggest_split(self.H, self.nh * self.d, T),
+        return dict(qkv=c.suggest_split(self._n_qkv, self.H, T), o=c.suggest_split(self.H, self.nh * self.d, T),
                     gu=c.suggest_split(self.I, self.H, T, True), d=c.suggest_split(self.H, self.I, T))
 
     def _ws_floats(self, T, sp):
-        return max(sp["qkv"] * T * self.wqkv[0].shape[0] if sp["qkv"] > 1 else 0, sp["o"] * T * self.H if sp["o"] > 1 else 0,
+        return max(sp["qkv"] * T * self._n_qkv if sp["qkv"] > 1 else 0, sp["o"] * T * self.H if sp["o"] > 1 else 0,
                    sp["gu"] * T * 2 * self.I if T <= 128 else 0, sp["d"] * T * self.H if sp["d"] > 1 else 0, 1)
 
     def _w4_splits(self, T):
@@ -375,7 +462,7 @@ class ChatTSForCausalLM:
         w4, c = self.w4, self.ctx
         if w4["splits"] is not None:
             return w4["splits"]
-        return dict(qkv=c.gemm_w4_mma_suggest_split(self.wqkv[0].shape[0], self.H, T), o=c.gemm_w4_mma_suggest_split(self.H, self.nh * self.d, T),
+        return dict(qkv=c.gemm_w4_mma_suggest_split(self._n_qkv, self.H, T), o=c.gemm_w4_mma_suggest_split(self.H, self.nh * self.d, T),
                     gu=c.gemm_w4_mma_suggest_split(2 * self.I, self.H, T), d=c.gemm_w4_mma_suggest_split(self.H, self.I, T))
 
     def _layers(self, st, T, attend):
@@ -383,25 +470,38 @@ class ChatTSForCausalLM:
         c, sp, eps = self.ctx, st.splits, self.eps
         I, H = self.I, self.H
         c.reduce_residual_rmsnorm(None, 0, st.h, None, self.ln1[0], eps, st.xn, t=T)
-        fused = self.use_fused_decode and T <= 32 and st.k_lin is None                            # decode states only
+        fp8 = self.fp8
+        fused = self.use_fused_decode and T <= 32 and st.k_lin is None and fp8 is None             # decode states only
         # decode-sized steps: every weight-streaming GEMM names the weight its successor will stream, and prefetches the head of it
         # into L2 once its own last tile is requested (cts_gemm_args.next_*): HBM keeps streaming through the kernel boundaries
-        nb = self.next_prefetch_bytes if (T <= 32 and st.k_lin is None) else 0
+        nb = self.next_prefetch_bytes if (T <= 32 and st.k_lin is None and fp8 is None) else 0
         # W4A16: decode-sized steps stream the 4-bit codes (every projection through the split-K partial path with the W4 split factors)
         w4 = self.w4 if (self.w4 is not None and T <= 32 and st.k_lin is None and not fused) else None
         if w4 is not None:
             sp = self._w4_splits(T)
+        # FP8: decode-sized steps stream the codes the same way; every other step dequantises each projection just before its GEMM
+        f8 = fp8 is not None and T <= 32 and st.k_lin is None
+        if f8:
+            sp = self._fp8_splits(T)
+        dense = {"qkv": self.wqkv, "o": self.wo, "gu": self.wgu, "d": self.wd}
 
-        def proj(kind, l, x, w, split, **kw):
-            """fp32 split-K partials of one projection into st.ws: from the packed 4-bit weight when attached, else from the dense one."""
+        def W(kind, l):
+            """The 16-bit weight of a projection for cts_gemm (FP8 model: dequantised into the scratch matrix now)."""
+            return dense[kind][l] if fp8 is None else self._fp8_dense(fp8[kind][l])
+
+        def proj(kind, l, x, split, **kw):
+            """fp32 split-K partials of one projection into st.ws: from the packed 4-bit / FP8 weight when attached, else from the dense one."""
             if w4 is not None and w4["kernel"] == "mma":
                 qwf, szp, n_out = w4[kind][l]
                 c.gemm_w4_mma(x, qwf, szp, n_out, w4["group_size"], st.ws, split, t=T)
             elif w4 is not None:
                 qw, sc, zp = w4[kind][l]
                 c.gemm_w4(x, qw, sc, zp, w4["group_size"], st.ws, split, t=T)
+            elif f8:
+                qw, sc, k = fp8[kind][l]
+                c.gemm_fp8(x, qw, sc, k, st.ws, split, t=T)
             else:
-                c.gemm(x, w, st.ws, epilogue=EPI_PARTIAL_F32, split_k=split, t=T, **kw)
+                c.gemm(x, W(kind, l), st.ws, epilogue=EPI_PARTIAL_F32, split_k=split, t=T, **kw)
 
         def nxt(w, split):
             return dict(next_w=w, next_split=split, next_bytes=nb) if nb > 0 else {}
@@ -458,40 +558,40 @@ class ChatTSForCausalLM:
                     c.reduce_residual_rmsnorm(None, 0, st.h, None, nw, eps, st.xn, t=T)
                 continue
             # ---- QKV projection + bias + RoPE + KV write
-            if sp["qkv"] > 1 or w4 is not None:
-                proj("qkv", l, st.xn, self.wqkv[l], sp["qkv"], **nxt(self.wo[l], sp["o"]))
+            if sp["qkv"] > 1 or w4 is not None or f8:
+                proj("qkv", l, st.xn, sp["qkv"], **nxt(self.wo[l], sp["o"]))
                 c.qkv_rope_cache(st.ws, True, sp["qkv"], self.bqkv[l], st.positions, self.cos, self.sin, st.slot_map, st.q, kc, vc,
                                  st.k_lin, st.v_lin, T, self.nh, self.nkv, self.d, self.page_size, self.qn[l], self.kn[l], eps)
             else:
-                c.gemm(st.xn, self.wqkv[l], st.qkv, bias=self.bqkv[l], epilogue=EPI_NONE, t=T, **nxt(self.wo[l], sp["o"]))
+                c.gemm(st.xn, W("qkv", l), st.qkv, bias=self.bqkv[l], epilogue=EPI_NONE, t=T, **nxt(self.wo[l], sp["o"]))
                 c.qkv_rope_cache(st.qkv, False, 1, None, st.positions, self.cos, self.sin, st.slot_map, st.q, kc, vc,
                                  st.k_lin, st.v_lin, T, self.nh, self.nkv, self.d, self.page_size, self.qn[l], self.kn[l], eps)
             attend(l)
             # ---- o_proj + residual + post-attention RMSNorm
             if self.tp_size > 1:
-                self._tp_row_parallel(st, T, st.ao, self.wo[l], self.ln2[l], 0, sp["o"], nxt(self.wgu[l], sp["gu"]))
-            elif sp["o"] > 1 or w4 is not None:
-                proj("o", l, st.ao, self.wo[l], sp["o"], **nxt(self.wgu[l], sp["gu"]))
+                self._tp_row_parallel(st, T, st.ao, fp8["o"][l] if f8 else W("o", l), self.ln2[l], 0, sp["o"], nxt(self.wgu[l], sp["gu"]))
+            elif sp["o"] > 1 or w4 is not None or f8:
+                proj("o", l, st.ao, sp["o"], **nxt(self.wgu[l], sp["gu"]))
                 c.reduce_residual_rmsnorm(st.ws, sp["o"], st.h, st.h, self.ln2[l], eps, st.xn, t=T)
             else:
-                c.gemm(st.ao, self.wo[l], st.h, residual=st.h, epilogue=EPI_RESIDUAL, t=T, **nxt(self.wgu[l], sp["gu"]))
+                c.gemm(st.ao, W("o", l), st.h, residual=st.h, epilogue=EPI_RESIDUAL, t=T, **nxt(self.wgu[l], sp["gu"]))
                 c.reduce_residual_rmsnorm(None, 0, st.h, None, self.ln2[l], eps, st.xn, t=T)
             # ---- gate/up + SwiGLU
             if T > 128:
-                c.gemm(st.xn, self.wgu[l], st.act, epilogue=EPI_SWIGLU_IL, t=T)          # persistent, SwiGLU fused in the tile
+                c.gemm(st.xn, W("gu", l), st.act, epilogue=EPI_SWIGLU_IL, t=T)          # persistent, SwiGLU fused in the tile
             else:
-                proj("gu", l, st.xn, self.wgu[l], sp["gu"], **nxt(self.wd[l], sp["d"]))
+                proj("gu", l, st.xn, sp["gu"], **nxt(self.wd[l], sp["d"]))
                 c.reduce_swiglu(st.ws, sp["gu"], T, I, st.act, interleaved=True)
             # ---- down_proj + residual + next layer's input RMSNorm (or the final norm)
             nw = self.ln1[l + 1] if l + 1 < self.L else self.final_norm
             after = nxt(self.wqkv[l + 1], sp["qkv"]) if l + 1 < self.L else nxt(self.lm_head, 1)
             if self.tp_size > 1:
-                self._tp_row_parallel(st, T, st.act, self.wd[l], nw, 1, sp["d"], after)
-            elif sp["d"] > 1 or w4 is not None:
-                proj("d", l, st.act, self.wd[l], sp["d"], **after)
+                self._tp_row_parallel(st, T, st.act, fp8["d"][l] if f8 else W("d", l), nw, 1, sp["d"], after)
+            elif sp["d"] > 1 or w4 is not None or f8:
+                proj("d", l, st.act, sp["d"], **after)
                 c.reduce_residual_rmsnorm(st.ws, sp["d"], st.h, st.h, nw, eps, st.xn, t=T)
             else:
-                c.gemm(st.act, self.wd[l], st.h, residual=st.h, epilogue=EPI_RESIDUAL, t=T, **after)
+                c.gemm(st.act, W("d", l), st.h, residual=st.h, epilogue=EPI_RESIDUAL, t=T, **after)
                 c.reduce_residual_rmsnorm(None, 0, st.h, None, nw, eps, st.xn, t=T)
 
     def _tp_row_parallel(self, st, T, x, w, norm_w, which, split, nxt=None):
@@ -499,9 +599,12 @@ class ChatTSForCausalLM:
         residual + norm.  Decode-sized T: ONE kernel over NVLink peer memory (cts_peer_allreduce_residual_rmsnorm: each
         CTA reduces its token's local split-K partials into the symmetric buffer, signals, pulls the peers' rows; the
         buffers alternate between o_proj (0) and down_proj (1)).  Large prefill T: NCCL (bandwidth-bound) -- fp32 reduce-scatter over token
-        shards + all-gather of the rounded result by default, see the branches below."""
+        shards + all-gather of the rounded result by default, see the branches below.  ``w``: the 16-bit weight, or the (codes, scales, k)
+        of an FP8 projection for a decode-sized step (cts_gemm_fp8)."""
         c = self.ctx
         big = split == 1 and not (self.peer is not None and T <= self.peer_tokens)
+        if isinstance(w, tuple) and big:
+            w = self._fp8_dense(w)
         if big and self.tp_prefill_exchange == "16bit":
             # Opt-in (CTS_TP_PREFILL_EXCHANGE=16bit): every rank rounds its projection to the model dtype and NCCL sums the ranks' outputs
             # in that dtype -- what vLLM's RowParallelLinear does (qwen2.py:100-116 / 168-174) -- half the bytes of the fp32 all-reduce.
@@ -526,7 +629,10 @@ class ChatTSForCausalLM:
             st.h[:T].add_(st.tp_proj[:T])                         # residual add in the model dtype, as the fused tail does
             c.reduce_residual_rmsnorm(None, 0, st.h, st.h, norm_w, self.eps, st.xn, t=T)
             return
-        c.gemm(x, w, st.ws, epilogue=EPI_PARTIAL_F32, split_k=split, t=T, **(nxt or {}))
+        if isinstance(w, tuple):
+            c.gemm_fp8(x, w[0], w[1], w[2], st.ws, split, t=T)
+        else:
+            c.gemm(x, w, st.ws, epilogue=EPI_PARTIAL_F32, split_k=split, t=T, **(nxt or {}))
         if self.peer is not None and T <= self.peer_tokens and self.use_peer_ll:
             c.peer_allreduce_ll(st.ws, split, self.peer.partials[which], self.peer.part_bytes, self.peer.state, self.tp_rank, self.tp_size,
                                 self.peer.max_batch, st.h, st.h, norm_w, self.eps, st.xn, T)
@@ -557,14 +663,17 @@ class ChatTSForCausalLM:
             st.tp_proj = torch.empty(tp_pad, self.H, device=dev, dtype=dt)
             st.tp_shard32 = torch.empty(ct * self.H, device=dev, dtype=torch.float32)
             st.tp_shard16 = torch.empty(ct * self.H, device=dev, dtype=dt)
-        st.qkv = torch.empty(T, self.wqkv[0].shape[0], device=dev, dtype=dt) if st.splits["qkv"] == 1 else None
+        st.qkv = torch.empty(T, self._n_qkv, device=dev, dtype=dt) if st.splits["qkv"] == 1 else None
         ws_n = max(self._ws_floats(T, st.splits), T * self.H, tp_pad * self.H)
         if decode and self.w4 is not None and T <= 32:   # W4A16 decode: every projection through the partial path with the W4 split factors
             sp = self._w4_splits(T)
-            ws_n = max(ws_n, sp["qkv"] * T * self.wqkv[0].shape[0], sp["o"] * T * self.H, sp["gu"] * T * 2 * self.I, sp["d"] * T * self.H)
+            ws_n = max(ws_n, sp["qkv"] * T * self._n_qkv, sp["o"] * T * self.H, sp["gu"] * T * 2 * self.I, sp["d"] * T * self.H)
+        if decode and self.fp8 is not None and T <= 32:  # FP8 decode: every projection through the partial path with the FP8 split factors
+            sp = self._fp8_splits(T)
+            ws_n = max(ws_n, sp["qkv"] * T * self._n_qkv, sp["o"] * T * self.H, sp["gu"] * T * 2 * self.I, sp["d"] * T * self.H)
         if decode and self.use_native_step:          # cts_decoder_step always takes the split-K partial path (also at factor 1)
             sp = st.splits
-            ws_n = max(ws_n, sp["qkv"] * T * self.wqkv[0].shape[0], sp["o"] * T * self.H, sp["gu"] * T * 2 * self.I, sp["d"] * T * self.H)
+            ws_n = max(ws_n, sp["qkv"] * T * self._n_qkv, sp["o"] * T * self.H, sp["gu"] * T * 2 * self.I, sp["d"] * T * self.H)
         st.ws = torch.empty(ws_n, device=dev, dtype=torch.float32)                           # split-K partials [S, T, N]
         st.positions = torch.zeros(T, device=dev, dtype=torch.int32)
         st.slot_map = torch.zeros(T, device=dev, dtype=torch.int32)
@@ -728,10 +837,10 @@ class ChatTSForCausalLM:
         return st
 
     def _native_ok(self, B):
-        return self.use_native_step and self.tp_size == 1 and B <= 128 and not self._chain_ok(B) and self.w4 is None
+        return self.use_native_step and self.tp_size == 1 and B <= 128 and not self._chain_ok(B) and self.w4 is None and self.fp8 is None
 
     def _chain_ok(self, B):
-        return (self.w4 is None and self.use_chain and self.tp_size == 1 and B <= 32 and self.H % 64 == 0 and self.H // 64 <= 192 and self.I % 64 == 0)
+        return (self.w4 is None and self.fp8 is None and self.use_chain and self.tp_size == 1 and B <= 32 and self.H % 64 == 0 and self.H // 64 <= 192 and self.I % 64 == 0)
 
     def _decode_layers_chain(self, st, attend):
         """Decode layers with the persistent chain kernel: per layer ONE attention launch + ONE chain launch
@@ -779,7 +888,7 @@ class ChatTSForCausalLM:
             self._decode_layers_chain(st, attend)
         else:
             self._layers(st, B, attend)
-        nb = self.next_prefetch_bytes if B <= 32 else 0
+        nb = self.next_prefetch_bytes if (B <= 32 and self.fp8 is None) else 0
         c.gemm(st.xn, self.lm_head, st.logits, epilogue=EPI_NONE, t=B,
                **(dict(next_w=self.wqkv[0], next_split=st.splits["qkv"], next_bytes=nb) if nb > 0 else {}))
         if sample and self.peer is not None:

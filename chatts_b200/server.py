@@ -348,7 +348,7 @@ def create_app(llm, served_model_name="chatts", batch_window_ms=5.0, max_ts_per_
     return app
 
 
-def main():
+def parse_args(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", default=None, help="checkpoint directory; default: synthetic ChatTS-14B weights + byte tokenizer")
     ap.add_argument("--served-model-name", default="chatts")
@@ -362,7 +362,13 @@ def main():
     ap.add_argument("--scheduler", default="batch", choices=["batch", "continuous"],
                     help="batch: micro-batches run to completion (sampling supported); continuous: iteration-level batching, greedy")
     ap.add_argument("--steps-per-round", type=int, default=4, help="continuous scheduler: decode steps between two host reads")
-    args = ap.parse_args()
+    ap.add_argument("--quantization", default=None, choices=["fp8"],
+                    help="fp8: decoder projections quantised to FP8 (e4m3, per-output-channel scales) at load time")
+    return ap.parse_args(argv)
+
+
+def main():
+    args = parse_args()
     import uvicorn
     from .vllm_compat import LLM
     limit = int(dict(kv.split("=") for kv in args.limit_mm_per_prompt.split(",")).get("timeseries", MAX_TS_DEFAULT))
@@ -371,7 +377,7 @@ def main():
         from transformers import AutoTokenizer
         tok = AutoTokenizer.from_pretrained(args.model, trust_remote_code=True)
     llm = LLM(model=args.model, tokenizer=tok, dtype=args.dtype, max_model_len=args.max_model_len, max_num_seqs=args.max_num_seqs,
-              limit_mm_per_prompt={"timeseries": limit})
+              limit_mm_per_prompt={"timeseries": limit}, quantization=args.quantization)
     uvicorn.run(create_app(llm, args.served_model_name, args.batch_window_ms, limit, args.scheduler, args.steps_per_round),
                 host=args.host, port=args.port)
 

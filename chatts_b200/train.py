@@ -75,6 +75,9 @@ class LoraTrainer:
                  weight_decay=0.0, max_grad_norm=1.0, seed=0, init_b_std=0.0, group=None, adapters=None):
         if model.tp_size != 1:
             raise ValueError("LoraTrainer is data parallel: build the model with tp_size=1 on every rank")
+        if model.fp8 is not None:
+            raise ValueError("LoraTrainer on an FP8 model: training reads the 16-bit projection weights, which quantize_fp8() freed -- "
+                             "train and merge on the 16-bit model, then quantize")
         if not 1 <= int(r) <= 64:
             raise ValueError("LoRA rank must be in [1, 64]")
         self.model, self.ctx = model, model.ctx

@@ -141,14 +141,18 @@ def _make_llm(**kw):
 class LLM:
     def __init__(self, model=None, tokenizer=None, config=None, state_dict=None, tensor_parallel_size=1, dtype="bfloat16",
                  max_model_len=2048, max_num_seqs=32, limit_mm_per_prompt=None, trust_remote_code=True, seed=1234,
-                 distributed_backend="nccl", **kw):
+                 distributed_backend="nccl", quantization=None, **kw):
         """tensor_parallel_size = k > 1 (every caller of the reference passes it: demo/demo_vllm.py:30, llm_utils.py:153-154):
           * under torchrun / an initialised process group of k ranks the engine ATTACHES: every rank constructs the LLM and makes the
             same generate() calls (rank r holds shard r);
           * otherwise the constructor SPAWNS k - 1 worker processes (one per GPU, as vLLM's multiprocessing executor does,
             README.md:141) that build their shards and mirror every generate() call of this process (rank 0) -- the model must then
-            be named by a path or by config + seed (a ChatTSForCausalLM instance cannot be sent to another process)."""
+            be named by a path or by config + seed (a ChatTSForCausalLM instance cannot be sent to another process).
+        quantization: None (the checkpoint's 16-bit weights) or "fp8" (vLLM's weight-only FP8: ChatTSForCausalLM.quantize_fp8 at load time,
+        on every rank)."""
         import os
+        if quantization not in (None, "fp8"):
+            raise ValueError(f"quantization={quantization!r}: supported are None and 'fp8'")
         self._tp_procs, self._tp_driver = [], False
         tp = int(tensor_parallel_size or 1)
         tp_kw = {}
@@ -175,7 +179,7 @@ class LLM:
                 port = _free_port()
                 child_kw = dict(model=model, tokenizer=tokenizer, config=config, tensor_parallel_size=tp, dtype=dtype, max_model_len=max_model_len,
                                 max_num_seqs=max_num_seqs, limit_mm_per_prompt=limit_mm_per_prompt, seed=seed,
-                                distributed_backend=distributed_backend, **kw)
+                                distributed_backend=distributed_backend, quantization=quantization, **kw)
                 ctx = mp.get_context("spawn")
                 for r in range(1, tp):
                     pr = ctx.Process(target=_tp_worker, args=(r, tp, port, distributed_backend, _make_llm, child_kw), daemon=True)
@@ -193,12 +197,15 @@ class LLM:
         if isinstance(model, ChatTSForCausalLM):
             self.model = model
         elif isinstance(model, str):
-            self.model = ChatTSForCausalLM.from_pretrained(model, torch_dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs, **tp_kw)
+            self.model = ChatTSForCausalLM.from_pretrained(model, torch_dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs,
+                                                           quantization=quantization, **tp_kw)
         else:
             cfg = config or ChatTSConfig.chatts_14b()
             self.model = (ChatTSForCausalLM(cfg, state_dict, dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs, **tp_kw)
                           if state_dict is not None else
                           ChatTSForCausalLM.from_synthetic(cfg, seed=seed, dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs, **tp_kw))
+        if quantization == "fp8" and self.model.fp8 is None:
+            self.model.quantize_fp8()
         cfg = self.model.config
         self.tokenizer = tokenizer or SimpleTokenizer(cfg.ts_token_start_index, cfg.pad_token_id, cfg.eos_token_id)
         self.processor = ChatTSProcessor(self.tokenizer, cfg, dtype=torch.float32)

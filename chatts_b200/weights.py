@@ -208,6 +208,61 @@ def repack_w4_mma(qw, sc, zp, group_size=128):
     return qwf, pair
 
 
+# --------------------------------------------------------------------------------------------------
+# FP8 weight-only quantisation (ChatTSForCausalLM.quantize_fp8, vLLM's quantization="fp8"): e4m3 codes with one fp32 scale per output
+# feature, s_n = max|W[n, :]| / 448 over the full checkpoint row, codes = RNE(W / s_n).  Per-row scales commute with stacking rows, so
+# quantising q, k, v (or gate, up) separately and fusing afterwards gives the same codes as quantising the fused matrix.
+# --------------------------------------------------------------------------------------------------
+FP8_E4M3_MAX = 448.0
+FP8_MMA_TILE = 256         # features per chunk of the fragment-major layout (csrc/gemm_fp8.cu: kTileN)
+
+
+def fp8_row_scales(row_max):
+    """fp32 scales of rows whose largest magnitude is ``row_max``; an all-zero row gets scale 1 (its codes are all 0)."""
+    m = row_max.to(torch.float32)
+    return torch.where(m > 0, m / FP8_E4M3_MAX, torch.ones_like(m))
+
+
+def quantize_fp8_rows(w, row_max=None, name="weight"):
+    """w [out, in] -> (codes uint8 [out, in]: float8_e4m3fn bit patterns, round to nearest even; scales fp32 [out]).  ``row_max``:
+    max |W[n, :]| over the FULL row when ``w`` holds a K-slice of it (tensor parallelism), default the rows of ``w``."""
+    if not bool(torch.isfinite(w).all()):
+        raise ValueError(f"quantize_fp8: {name} holds non-finite values")
+    if row_max is None:
+        row_max = w.abs().amax(1).to(torch.float32)
+    s = fp8_row_scales(row_max)
+    q = (w.to(torch.float32) / s[:, None]).clamp_(-FP8_E4M3_MAX, FP8_E4M3_MAX).to(torch.float8_e4m3fn)
+    return q.view(torch.uint8), s
+
+
+def dequantize_fp8(codes, scales, dtype):
+    """Host statement of cts_fp8_dequant: dtype(fp32(e4m3(codes)) * s_n), one rounding."""
+    return (codes.view(torch.float8_e4m3fn).to(torch.float32) * scales.to(torch.float32)[:, None]).to(dtype)
+
+
+def pack_fp8_mma(codes):
+    """Row layout (uint8 [out, in], in % 64 == 0) -> the fragment-major layout cts_gemm_fp8 / cts_fp8_dequant read
+    (include/chatts_b200.h: cts_gemm_fp8_args): uint8 [ceil(out/256) * in/64 * 16384], chunk (tile, kb) = for m-tile m (16 features),
+    k16-step pair h, lane = 4 g + t: 16 bytes = k16 step 2h + kl (8 bytes each) x word j (4 bytes) x {row g, g + 8} x {k, k + 1} at
+    k = 64 kb + 16 (2h + kl) + 8 j + 2 t.  Features beyond ``out`` get code 0."""
+    n_out, n_in = codes.shape
+    assert n_in % 64 == 0, "the FP8 layout needs in_features % 64 == 0"
+    tiles = -(-n_out // FP8_MMA_TILE)
+    q = codes
+    if tiles * FP8_MMA_TILE != n_out:
+        q = torch.cat([q, torch.zeros(tiles * FP8_MMA_TILE - n_out, n_in, dtype=q.dtype, device=q.device)], 0)
+    # feature = 256 tile + 16 m + 8 b2 + g ; k = 64 kb + 32 h + 16 kl + 8 j + 2 t + b1
+    v = q.view(tiles, 16, 2, 8, n_in // 64, 2, 2, 2, 4, 2)          # [tile, m, b2, g, kb, h, kl, j, t, b1]
+    return v.permute(0, 4, 1, 5, 3, 8, 6, 7, 2, 9).contiguous().view(-1)   # [tile, kb, m, h, g, t, kl, j, b2, b1]
+
+
+def unpack_fp8_mma(packed, n_out, n_in):
+    """Inverse of pack_fp8_mma: uint8 [n_out, n_in]."""
+    tiles = -(-n_out // FP8_MMA_TILE)
+    v = packed.view(tiles, n_in // 64, 16, 2, 8, 4, 2, 2, 2, 2)    # [tile, kb, m, h, g, t, kl, j, b2, b1]
+    return v.permute(0, 2, 8, 4, 1, 3, 6, 7, 5, 9).reshape(tiles * FP8_MMA_TILE, n_in)[:n_out]
+
+
 def dequantize_gptq(sd, quant_cfg=None, dtype=torch.bfloat16, scale_dtype=None):
     """Replace every ``<name>.{qweight,qzeros,scales[,g_idx]}`` group of a GPTQ checkpoint by ``<name>.weight``."""
     quant_cfg = quant_cfg or {}

@@ -528,6 +528,34 @@ typedef struct {
 int cts_gemm_w4_mma(cts_ctx* ctx, const cts_gemm_w4f_args* args, void* stream);
 int cts_gemm_w4_mma_suggest_split(cts_ctx* ctx, long long n, long long k, long long t);
 
+/* W8A16 decode GEMM for FP8 weights (ChatTSForCausalLM.quantize_fp8: e4m3 codes, one fp32 scale per output feature; csrc/gemm_fp8.cu:
+ * mma.sync with the codes converted in registers, persistent CTAs, the code stream by cp.async.bulk):
+ *   partial[s][t][n] = scales[n] * sum over split s of x[t][k] * e4m3(q[n][k])     (fp32 accumulate, the scale applied after it)
+ * 1 <= t <= 32; out = fp32 split-K partials [split_k, t, n] exactly as cts_gemm(CTS_EPI_PARTIAL_F32) writes them.
+ *   qw     uint8, ceil(n / 256) * (k / 64) chunks of 16384 bytes: chunk (tile, kb) holds features [256 tile, 256 tile + 256) x K [64 kb, 64 kb + 64)
+ *          as mma.m16n8k16 A fragments -- byte ((2 m + ks / 2) * 32 + lane) * 16 + 8 (ks % 2) + 4 j + b, for m-tile m (16 features),
+ *          lane (g = lane / 4, t = lane % 4), k16 step ks, holds the code of feature 16 m + g + 8 (b / 2) at k = 16 ks + 2t + 8 j + b % 2
+ *          (chatts_b200/weights.py:pack_fp8_mma); features beyond n: code 0
+ *   scales fp32 [n]
+ * k must be a multiple of 64; split_k <= k / 64 (the K ranges of the partials are cut at multiples of 64). */
+typedef struct {
+  const void* qw; const float* scales; const void* x; float* out;
+  long long n, k, t, x_ld;
+  int split_k, dtype, reserved0, reserved1;
+} cts_gemm_fp8_args;
+int cts_gemm_fp8(cts_ctx* ctx, const cts_gemm_fp8_args* args, void* stream);
+int cts_gemm_fp8_suggest_split(cts_ctx* ctx, long long n, long long k, long long t);
+
+/* The same weight as a row-major 16-bit matrix for prefill-sized steps: out[f * out_ld + k] = dtype(fp32(e4m3(q[f][k])) * scales[f])
+ * (one rounding), f < n, from the layout of cts_gemm_fp8_args.  out 16-byte aligned, out_ld >= k a multiple of 8, k a multiple of 64.
+ * Safe to follow with a cts_gemm that takes `out` as its weight: the next kernel on the stream starts after `out` is complete. */
+typedef struct {
+  const void* qw; const float* scales; void* out;
+  long long n, k, out_ld;
+  int dtype, reserved;
+} cts_fp8_dequant_args;
+int cts_fp8_dequant(cts_ctx* ctx, const cts_fp8_dequant_args* args, void* stream);
+
 /* Repetition penalty (transformers RepetitionPenaltyLogitsProcessor; generation_config.json of a checkpoint may set it): the set of
  * token ids that occur in a row's sequence is a bit mask seen[batch][words_per_row] (words_per_row >= ceil(vocab / 32), zeroed by the
  * caller).  _mark sets the bits of n (row, token) pairs (rows NULL: pair i belongs to row i -- the new token of every sequence after

@@ -5,6 +5,7 @@ Unlike tools/dryrun_train_gpu_tests.py (which checks the TEST LOGIC against the 
 TEST INFRASTRUCTURE ONLY.
 
     python tools/shim_gpu_tests.py [--quick] [pytest args]
+    python tools/shim_gpu_tests.py tests/test_gpu_fp8.py [-k cases]      # only the named files (default cases: their SELECT entry)
 """
 import functools
 import os
@@ -60,9 +61,10 @@ torch.cuda.current_device = lambda: 0
 torch.cuda.is_current_stream_capturing = lambda: False
 
 from tests.cuda_on_cpu.shim import shim_context  # noqa: E402
+from tests.cuda_on_cpu.fp8 import attach as _attach_fp8  # noqa: E402
 import tests.gpu_util as gu  # noqa: E402
 
-_ctx = shim_context()
+_ctx = _attach_fp8(shim_context())                      # + the FP8 kernels (their own shim library on the same runtime)
 from tests.cabi_double import TorchDouble as _TD  # noqa: E402
 _dbl = _TD()
 # HYBRID context for the whole-step tests: every entry point whose source is in the shim build runs that source; the others (wgmma
@@ -113,6 +115,8 @@ SELECT = {
     "test_gpu_attention.py": None,                       # calibration: HMMA prefill, TMA paged decode (ldmatrix / mma.sync)
     "test_gpu_zz_d_attn_bwd_wgmma.py": None,             # wgmma attention backward (K-major and MN-major operands, register-A MMAs)
     "test_gpu_w4.py": "not (27648 or 13824 or 7168)",    # both W4A16 kernels (wgmma operand path; registers + mma.sync over the persistent schedule), small shapes
+    # the FP8 decode GEMM (every code at every fragment position, partials at the small shapes) and the dequantisation kernel
+    "test_gpu_fp8.py": "every_code or suggested or (partials and (704 or 1408 or 256-256 or 200 or 528)) or (dequant and 200-704)",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
@@ -134,6 +138,10 @@ if __name__ == "__main__":
         extra.remove("--quick")
         SELECT = QUICK
     print("entry points running from kernel source:", " ".join(sorted(_shim_native)))
+    named = [a for a in extra if a.endswith(".py")]
+    if named:
+        extra = [a for a in extra if a not in named]
+        SELECT = {os.path.basename(f): SELECT.get(os.path.basename(f)) for f in named}
     rc = 0
     for f, k in SELECT.items():
         args = [os.path.join(ROOT, "tests", f), "-q", "-p", "no:cacheprovider", "--runxfail", "-m", "gpu", "-x"] + (["-k", k] if k and "-k" not in extra else []) + extra

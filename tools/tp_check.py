@@ -1,5 +1,6 @@
-"""torchrun --nproc-per-node 2 tools/tp_check.py : tensor-parallel path (NCCL prefill all-reduce + fused peer-memory
-decode all-reduce) against the single-GPU path on the same weights."""
+"""torchrun --nproc-per-node 2 tools/tp_check.py [--fp8] : tensor-parallel path (NCCL prefill all-reduce + fused peer-memory
+decode all-reduce) against the single-GPU path on the same weights.  --fp8: both models quantize_fp8()'d (the row maximum of the K-sliced
+o_proj / down_proj all-reduced over the ranks, so both hold the same FP8 weights)."""
 import os
 import sys
 
@@ -26,7 +27,10 @@ def main():
     x = np.arange(256)
     enc = proc(text=["A <ts><ts/> then B <ts><ts/> ?", "plain text only prompt"], timeseries=[np.sin(x / 10) * 5, x[:90] * 0.1],
                padding=True, return_tensors="pt")
+    fp8 = "--fp8" in sys.argv[1:]
     tp = ChatTSForCausalLM(cfg, sd, dtype=dt, tp_rank=rank, tp_size=world, max_batch=4, max_seq_len=512, page_size=16)
+    if fp8:
+        tp.quantize_fp8()
     # a prefill whose total token count is NOT a multiple of the world size and above the peer-memory path's limit: the NCCL exchange of the
     # row-parallel projections (fp32 reduce-scatter over padded token shards + 16-bit all-gather, model.py:_tp_row_parallel)
     filler = "the quick brown fox jumps over the lazy dog " * 3
@@ -43,12 +47,14 @@ def main():
     ok = True
     if rank == 0:
         ref = ChatTSForCausalLM(cfg, sd, dtype=dt, max_batch=4, max_seq_len=512, page_size=16)
+        if fp8:
+            ref.quantize_fp8()
         lg = ref.forward(enc["input_ids"], enc["attention_mask"], enc["timeseries"]).logits[:, 0].float().cpu()
         ids = ref.generate(**enc, max_new_tokens=24, ignore_eos=True)
         err = float((lg_tp - lg).abs().max() / lg.abs().max())
         S = enc["input_ids"].shape[1]
         agree = [int(next((i for i in range(24) if ids[b, S + i] != ids_tp[b, S + i]), 24)) for b in range(2)]
-        print(f"[tp_check] world={world} logits rel err vs single GPU {err:.3e}; greedy agreement {agree}/24", flush=True)
+        print(f"[tp_check] world={world} fp8={int(fp8)} logits rel err vs single GPU {err:.3e}; greedy agreement {agree}/24", flush=True)
         ok = err < 2e-2
     # all ranks must hold identical tokens (the fused all-reduce sums in rank order on every rank)
     t = ids_tp.cuda()
