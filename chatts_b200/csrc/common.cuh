@@ -20,13 +20,17 @@ struct cts_ctx {
   void* scratch;
   size_t scratch_bytes;
   PFN_cuTensorMapEncodeTiled_v12000 encode_tiled;
-  int l2_prefetch_mb;   // tuning knob (CTS_L2_PREFETCH_MB): weight bytes a decode GEMM prefetches into L2 while it waits
+  int l2_prefetch_mb;   // CTS_L2_PREFETCH_MB=-1: the persistent prefill GEMM walks its tiles feature-fastest instead of in L2 groups (A/B testing)
   int no_persistent_gemm;     // CTS_NO_PERSISTENT_GEMM=1: A/B switch back to the one-tile-per-CTA kernel for big T
   int norm_cluster;           // CTS_NORM_CLUSTER: max thread-block-cluster size of the decode RMSNorm kernel (default 8)
   int decode_stages;    // tuning knob (CTS_DECODE_SMEM_KB): shared-memory budget per CTA of the decode GEMM
   int no_ts_fused;      // CTS_TS_FUSED=0: the TS encoder always takes the multi-launch path (A/B testing)
   int no_next_prefetch; // CTS_NEXT_PREFETCH=0: ignore the next-GEMM weight prefetch hints (A/B testing)
   int next_prefetch_mb; // CTS_NEXT_PREFETCH_MB (default 0 = off): budget of the hint the C++ step executor passes (model.py passes its own)
+  int no_stream_gemm;   // CTS_NO_STREAM_GEMM=1: decode-sized GEMMs take gemm_tn_kernel instead of gemm_stream_kernel (reference / A/B runs)
+  int stream_ctas;      // tuning knobs of gemm_stream_kernel: resident CTAs per SM (CTS_STREAM_CTAS),
+  int stream_rows;      // weight rows per tile, 64 or 128 (CTS_STREAM_ROWS),
+  int stream_kblocks;   // 64-wide K blocks per ring slot, 1 / 2 / 4 (CTS_STREAM_KBLOCKS)
 };
 
 int cts_set_error(cts_ctx* ctx, int code, const char* fmt, ...);

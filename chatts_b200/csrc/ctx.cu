@@ -90,6 +90,14 @@ extern "C" int cts_ctx_create(int device, cts_ctx** out) {
   ctx->no_next_prefetch = (e6 && atoi(e6) == 0) ? 1 : 0;
   const char* e7 = getenv("CTS_NEXT_PREFETCH_MB");
   ctx->next_prefetch_mb = e7 ? atoi(e7) : 0;     // off by default: the prefetched bytes are read twice (once into L2, once by the GEMM)
+  const char* e9 = getenv("CTS_NO_STREAM_GEMM");
+  ctx->no_stream_gemm = e9 ? atoi(e9) : 0;
+  const char* e10 = getenv("CTS_STREAM_CTAS");
+  ctx->stream_ctas = e10 ? atoi(e10) : 2;
+  const char* e11 = getenv("CTS_STREAM_ROWS");
+  ctx->stream_rows = e11 ? atoi(e11) : 128;
+  const char* e12 = getenv("CTS_STREAM_KBLOCKS");
+  ctx->stream_kblocks = e12 ? atoi(e12) : 1;
   *out = ctx;
   return CTS_OK;
 }

@@ -43,7 +43,7 @@ struct GemmParams {
   int epilogue;
   float* splitk_ws;  // CTS_EPI_SPLITK_F32: fp32 [split_k, t, n] scratch
   int* tile_cnt;     // CTS_EPI_SPLITK_F32: arrival counter per output tile (zero-initialised, self-resetting)
-  int l2_prefetch;   // K blocks of W this CTA prefetches into L2 beyond the shared-memory ring while it waits (decode)
+  int l2_prefetch;   // persistent kernel: feature tiles per L2 group (0: feature-fastest order)
   int staged;        // 1: epilogue goes accumulator -> shared-memory output tile -> TMA store (big tiles)
   // next-GEMM weight prefetch (cts_gemm_args.next_*): units of the next launch = next_tiles x next_split, each reads K blocks
   // [kb_total' * z / split', ...) of the 128-row tile x; this grid prefetches the first next_pf blocks of every unit into L2
@@ -114,15 +114,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         const int kc = (kb0 + i) * kBK;
         tma_load_2d(st, &tm_w, &full_bar[i], kc, f0, CTS_L2_EVICT_FIRST);
         if (DUAL) tma_load_2d(st + kABytes, &tm_w2, &full_bar[i], kc, f0, CTS_L2_EVICT_FIRST);
-      }
-      // ... and, for the skinny decode GEMMs, the next K blocks straight into L2, so the HBM stream of this GEMM's
-      // weights keeps running while the (tiny) predecessor kernel holds the dependency.
-      {
-        const int npf = (nkb - npre) < p.l2_prefetch ? (nkb - npre) : p.l2_prefetch;
-        for (int i = npre; i < npre + npf; ++i) {
-          tma_prefetch_l2_2d(&tm_w, (kb0 + i) * kBK, f0);
-          if (DUAL) tma_prefetch_l2_2d(&tm_w2, (kb0 + i) * kBK, f0);
-        }
       }
       pdl_wait();   // activations are produced by the predecessor
       CTS_TRACE(CTS_TK_GEMM, 1);
@@ -308,6 +299,169 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   }
 
   if (threadIdx.x == 0) CTS_TRACE(CTS_TK_GEMM, 3);
+}
+
+// =================================================================================================================
+// Persistent weight-streaming kernel for decode-sized steps (t <= 32, one token tile), epilogues PARTIAL_F32 and NONE (split 1).
+// The work is a list of units = (weight-row tile of 64 H rows, K split), dealt round-robin to `ctas per SM x SMs` resident CTAs.  The
+// producer keeps one ring of `stages` slots full across unit boundaries; a slot holds KS consecutive 64-wide K blocks of the weight tile
+// (KS x 128 contiguous bytes of every row) and of the token tile.  The weight tiles of the first `stages` slots are requested before the
+// dependency wait (nobody writes weights), the token tiles and every store after it.  Each split covers the 64-wide K blocks
+// [kb_total s / split, kb_total (s + 1) / split) and each output is accumulated by the same m64nBNk16 wgmma sequence in ascending K as in
+// gemm_tn_kernel, so the fp32 partials are bit-identical to that kernel's at the same split factor; the ring depth, the tile height and
+// KS change only which bytes travel together.  The accumulator is stored straight from the fragment registers (eight consecutive
+// features per 32-byte sector), so the ring never stalls on an epilogue.
+//   warps 0..3 : MMA warpgroup + epilogue;  warp 4 : TMA producer (one lane)
+// =================================================================================================================
+constexpr int kSMaxStages = 16;
+constexpr int kSThreads = 160;
+
+struct StreamParams {
+  long long n, t, out_ld;
+  const void* bias;   // CTS_EPI_NONE only (may be null)
+  void* out;          // PARTIAL_F32: fp32 [split_k, t, n];  NONE: T [t, out_ld]
+  int kb_total, split_k, tiles, stages, epilogue;
+};
+
+template <int BN, int H, int KS> __host__ __device__ constexpr int stream_stage_bytes() { return KS * (H * 64 + BN) * kBK * 2; }
+
+template <typename T, int BN, int H, int KS>
+__global__ void __launch_bounds__(kSThreads, 1)
+gemm_stream_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x, const StreamParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t full_bar[kSMaxStages];
+  __shared__ uint64_t empty_bar[kSMaxStages];
+
+  constexpr int kRows = 64 * H;
+  constexpr int kWBlk = kRows * kBK * 2;       // one 64-wide K block of the weight tile
+  constexpr int kXBlk = BN * kBK * 2;          // ... and of the token tile
+  constexpr int kStage = stream_stage_bytes<BN, H, KS>();
+  constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
+
+  const uint32_t raw = smem_u32(smem_raw);
+  uint8_t* ring = smem_raw + (((raw + 1023u) & ~1023u) - raw);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int S = p.stages;
+  const int units = p.tiles * p.split_k;
+  auto unit = [&](int u, int& tile, int& split, int& kb0, int& kb1) {
+    tile = u % p.tiles;
+    split = u / p.tiles;
+    kb0 = (int)(((long long)p.kb_total * split) / p.split_k);
+    kb1 = (int)(((long long)p.kb_total * (split + 1)) / p.split_k);
+  };
+
+  pdl_trigger();
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_w);
+    tma_prefetch_desc(&tm_x);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 1);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp == 4) {
+    // ------------------------------ TMA producer ------------------------------
+    if (lane == 0) {
+      auto issue_w = [&](int s, int f0, int kb, int nb) {
+        mbar_expect_tx(&full_bar[s], (uint32_t)(nb * (kWBlk + kXBlk)));
+        uint8_t* st = ring + (size_t)s * kStage;
+        for (int b = 0; b < nb; ++b) tma_load_2d(st + b * kWBlk, &tm_w, &full_bar[s], (kb + b) * kBK, f0, CTS_L2_EVICT_FIRST);
+      };
+      int pre = 0;
+      for (int u = blockIdx.x; u < units && pre < S; u += gridDim.x) {
+        int tile, split, kb0, kb1;
+        unit(u, tile, split, kb0, kb1);
+        for (int kb = kb0; kb < kb1 && pre < S; kb += KS, ++pre) issue_w(pre, tile * kRows, kb, min(KS, kb1 - kb));
+      }
+      pdl_wait();   // activations are produced by the predecessor
+      int s = 0, n = 0;
+      uint32_t ph = 1u;                           // parity of the "slot is empty" phase waited for (a fresh barrier passes)
+      for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        int tile, split, kb0, kb1;
+        unit(u, tile, split, kb0, kb1);
+        for (int kb = kb0; kb < kb1; kb += KS, ++n) {
+          const int nb = min(KS, kb1 - kb);
+          if (n >= pre) {
+            mbar_wait(&empty_bar[s], ph);
+            issue_w(s, tile * kRows, kb, nb);
+          }
+          uint8_t* xs = ring + (size_t)s * kStage + KS * kWBlk;
+          for (int b = 0; b < nb; ++b) tma_load_2d(xs + b * kXBlk, &tm_x, &full_bar[s], (kb + b) * kBK, 0, CTS_L2_EVICT_LAST);
+          if (++s == S) { s = 0; ph ^= 1u; }
+        }
+      }
+    }
+  } else {
+    // ------------------------------ MMA warpgroup + epilogue ------------------------------
+    pdl_wait();   // the output buffers belong to predecessors until now
+    Acc128<BN> acc;                               // H == 1 uses the first m64 half only
+    float (&d)[2][BN / 2] = acc.d;
+    int s = 0;
+    uint32_t ph = 0u;
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
+      int tile, split, kb0, kb1;
+      unit(u, tile, split, kb0, kb1);
+      for (int kb = kb0; kb < kb1; kb += KS) {
+        const int nb = min(KS, kb1 - kb);
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t wa = smem_u32(ring + (size_t)s * kStage), xa = wa + KS * kWBlk;
+        if constexpr (H == 2) {
+#pragma unroll
+          for (int b = 0; b < KS; ++b)
+            if (b < nb) acc.template mma_kblock<kIsBf16>(wa + b * kWBlk, xa + b * kXBlk, kb == kb0 && b == 0);
+        } else {                                  // the same sequence on one m64 half
+          for (int i = 0; i < BN / 2; ++i) wgmma_fence_operand(d[0][i]);
+          wgmma_fence();
+#pragma unroll
+          for (int b = 0; b < KS; ++b) {
+            if (b < nb) {
+              const uint64_t ad = gmma_desc_k_sw128(wa + b * kWBlk), bd = gmma_desc_k_sw128(xa + b * kXBlk);
+#pragma unroll
+              for (int kk = 0; kk < 4; ++kk)
+                wgmma_m64k16<BN, kIsBf16>(d[0], ad + 2 * kk, bd + 2 * kk, (kb == kb0 && b == 0 && kk == 0) ? 0 : 1);
+            }
+          }
+          wgmma_commit();
+          for (int i = 0; i < BN / 2; ++i) wgmma_fence_operand(d[0][i]);
+        }
+        wgmma_wait<0>();
+        if (threadIdx.x == 0) mbar_arrive(&empty_bar[s]);
+        if (++s == S) { s = 0; ph ^= 1u; }
+      }
+      // ------------------------------ epilogue, from the fragment registers ------------------------------
+      const long long f0 = (long long)tile * kRows;
+      if (p.epilogue == CTS_EPI_PARTIAL_F32) {
+        float* dst = reinterpret_cast<float*>(p.out) + (long long)split * p.t * p.n;
+#pragma unroll
+        for (int h = 0; h < H; ++h)
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) {
+            const long long f = f0 + 64 * h + acc_row(i), t = acc_col(i);
+            if (t < p.t && f < p.n) dst[t * p.n + f] = d[h][i];
+          }
+      } else {
+        T* dst = reinterpret_cast<T*>(p.out);
+        const T* bias = reinterpret_cast<const T*>(p.bias);
+#pragma unroll
+        for (int h = 0; h < H; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const long long f = f0 + 64 * h + acc_row(2 * e);
+            const float bv = (bias != nullptr && f < p.n) ? DT<T>::to_f(bias[f]) : 0.f;
+#pragma unroll
+            for (int i = 2 * e; i < BN / 2; i += 4)
+#pragma unroll
+              for (int j = 0; j < 2; ++j) {
+                const long long t = acc_col(i + j);
+                if (t < p.t && f < p.n) dst[t * p.out_ld + f] = DT<T>::from_f(d[h][i + j] + bv);
+              }
+          }
+      }
+    }
+  }
 }
 
 // =================================================================================================================
@@ -552,13 +706,7 @@ int launch(cts_ctx* ctx, const cts_gemm_args* a, cudaStream_t stream) {
   if (stages < 2) stages = 2;
   p.stages = stages;
   p.staged = staged ? 1 : 0;
-  // decode (BN <= 32): prefetch up to ~64 MB of this GEMM's weights into L2 across the whole grid while waiting
   p.l2_prefetch = 0;
-  if (BN <= 32 && ctx->l2_prefetch_mb > 0) {
-    const long long ctas = cdiv_ll(a->n, kBM) * cdiv_ll(a->t, BN) * a->split_k;
-    const long long per = ((long long)ctx->l2_prefetch_mb << 20) / (ctas * kBM * kBK * 2 * (DUAL ? 2 : 1));
-    p.l2_prefetch = (int)(per > 64 ? 64 : per);
-  }
   if (staged && stages * kStage < 2 * BN * kBM * 2) stages = (2 * BN * kBM * 2 + kStage - 1) / kStage;
   p.stages = stages;
   const size_t acc_bytes = (size_t)acc_smem_bytes<BN>() * (DUAL ? 2 : 1);
@@ -569,6 +717,68 @@ int launch(cts_ctx* ctx, const cts_gemm_args* a, cudaStream_t stream) {
   dim3 grid((unsigned)cdiv_ll(a->n, kBM), (unsigned)cdiv_ll(a->t, BN), (unsigned)a->split_k);
   CTS_CUDA(ctx, launch_pdl(kern, grid, dim3(kThreads), smem, stream, 1, tm_w, tm_w2, tm_x, tm_next, tm_out, tm_res, p));
   return CTS_OK;
+}
+
+// The decode GEMM selection and shape of a context: read by ctx.cu at context creation.  The CPU shim's stand-in context has no such
+// fields; there the same variables (same defaults) are read from the environment at each launch.
+struct StreamCfg { int off, ctas, rows, kblocks; };
+static inline StreamCfg stream_cfg(const cts_ctx* ctx) {
+#ifndef CTS_HOST_SHIM
+  return {ctx->no_stream_gemm, ctx->stream_ctas, ctx->stream_rows, ctx->stream_kblocks};
+#else
+  auto env = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
+  return {env("CTS_NO_STREAM_GEMM", 0), env("CTS_STREAM_CTAS", 2), env("CTS_STREAM_ROWS", 128), env("CTS_STREAM_KBLOCKS", 1)};
+#endif
+}
+
+template <typename T, int BN, int H, int KS>
+int launch_stream(cts_ctx* ctx, const StreamCfg& cfg, const cts_gemm_args* a, cudaStream_t stream) {
+  const bool is_bf16 = a->dtype == CTS_BF16;
+  CUtensorMap tm_w, tm_x;
+  int rc = cts_make_tmap_2d(ctx, &tm_w, a->w, a->n, a->k, a->w_ld, 64 * H, is_bf16);
+  if (rc) return rc;
+  rc = cts_make_tmap_2d(ctx, &tm_x, a->x, a->t, a->k, a->x_ld, BN, is_bf16);
+  if (rc) return rc;
+  StreamParams p;
+  p.n = a->n; p.t = a->t; p.out_ld = a->out_ld;
+  p.bias = a->bias; p.out = a->out;
+  p.kb_total = (int)cdiv_ll(a->k, kBK);
+  p.split_k = a->split_k;
+  p.tiles = (int)cdiv_ll(a->n, 64 * H);
+  p.epilogue = a->epilogue;
+  // the ring takes whatever shared memory the resident CTAs of an SM leave each other
+  constexpr int kStage = stream_stage_bytes<BN, H, KS>();
+  const int ctas = cfg.ctas;
+  const int budget = (ctx->max_smem_optin + 1024) / ctas - 3 * 1024;
+  int stages = (budget - 1024) / kStage;
+  if (stages > kSMaxStages) stages = kSMaxStages;
+  if (stages < 2)
+    return cts_set_error(ctx, CTS_ERR_BAD_ARG, "cts_gemm: %d CTAs per SM leave room for fewer than two %d KB stages", ctas, kStage / 1024);
+  p.stages = stages;
+  const size_t smem = (size_t)stages * kStage + 1024;
+  auto kern = gemm_stream_kernel<T, BN, H, KS>;
+  CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+#ifndef CTS_HOST_SHIM
+  CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+#endif
+  const long long units = (long long)p.tiles * p.split_k;
+  long long grid = (long long)ctas * ctx->sm_count;
+  if (grid > units) grid = units;
+  CTS_CUDA(ctx, launch_pdl(kern, dim3((unsigned)grid), dim3(kSThreads), smem, stream, 1, tm_w, tm_x, p));
+  return CTS_OK;
+}
+
+template <typename T, int BN>
+int dispatch_stream(cts_ctx* ctx, const StreamCfg& c, const cts_gemm_args* a, cudaStream_t st) {
+  const int ks = c.kblocks;
+  if (c.rows == 64)
+    return ks == 1 ? launch_stream<T, BN, 1, 1>(ctx, c, a, st) : ks == 2 ? launch_stream<T, BN, 1, 2>(ctx, c, a, st) : launch_stream<T, BN, 1, 4>(ctx, c, a, st);
+  return ks == 1 ? launch_stream<T, BN, 2, 1>(ctx, c, a, st) : ks == 2 ? launch_stream<T, BN, 2, 2>(ctx, c, a, st) : launch_stream<T, BN, 2, 4>(ctx, c, a, st);
+}
+
+template <typename T>
+int dispatch_stream_bn(cts_ctx* ctx, const StreamCfg& c, const cts_gemm_args* a, cudaStream_t st) {
+  return a->t <= 16 ? dispatch_stream<T, 16>(ctx, c, a, st) : dispatch_stream<T, 32>(ctx, c, a, st);
 }
 
 template <typename T, bool DUAL>
@@ -603,6 +813,17 @@ extern "C" int cts_gemm(cts_ctx* ctx, const cts_gemm_args* a, void* stream) {
   CTS_CHECK_ARG(ctx, a->epilogue == CTS_EPI_PARTIAL_F32 || a->epilogue == CTS_EPI_SPLITK_F32 ||
                          a->out_ld >= (a->epilogue == CTS_EPI_SWIGLU_IL ? a->n / 2 : a->n), "out_ld smaller than n");
   cudaStream_t st = (cudaStream_t)stream;
+  // decode-sized launches that write fp32 partials (or, at split 1, the plain output) go to the persistent streaming kernel; row
+  // scatters, the dual SwiGLU accumulators, the in-kernel split-K reduction and launches carrying the next-GEMM L2 hint stay on
+  // gemm_tn_kernel (so does everything under CTS_NO_STREAM_GEMM=1)
+  const bool next_hint = a->next_w != nullptr && a->next_prefetch_bytes > 0;
+  const StreamCfg cfg = stream_cfg(ctx);
+  if (a->t <= 32 && (a->epilogue == CTS_EPI_PARTIAL_F32 || (a->epilogue == CTS_EPI_NONE && a->split_k == 1)) && a->row_map == nullptr &&
+      a->w2 == nullptr && !next_hint && !cfg.off) {
+    CTS_CHECK_ARG(ctx, cfg.ctas >= 1 && cfg.ctas <= 4 && (cfg.rows == 64 || cfg.rows == 128) && (cfg.kblocks == 1 || cfg.kblocks == 2 || cfg.kblocks == 4),
+                  "decode GEMM shape: CTS_STREAM_CTAS 1..4, CTS_STREAM_ROWS 64 or 128, CTS_STREAM_KBLOCKS 1, 2 or 4");
+    return a->dtype == CTS_BF16 ? dispatch_stream_bn<__nv_bfloat16>(ctx, cfg, a, st) : dispatch_stream_bn<__half>(ctx, cfg, a, st);
+  }
   CTS_CHECK_ARG(ctx, a->epilogue != CTS_EPI_SWIGLU_IL || (a->n % 128 == 0 && a->t > 128 && a->row_map == nullptr),
                 "CTS_EPI_SWIGLU_IL needs n % 128 == 0, t > 128 and no row_map (small t: CTS_EPI_PARTIAL_F32 + cts_reduce_swiglu)");
   const bool pers_epi = a->epilogue == CTS_EPI_NONE || a->epilogue == CTS_EPI_GELU || a->epilogue == CTS_EPI_RESIDUAL ||
@@ -622,9 +843,10 @@ extern "C" int cts_gemm(cts_ctx* ctx, const cts_gemm_args* a, void* stream) {
 extern "C" int cts_gemm_suggest_split(cts_ctx* ctx, long long n, long long k, long long t, int dual) {
   if (!ctx || n <= 0 || k <= 0 || t <= 0) return 1;
   const int bn = t <= 16 ? 16 : t <= 32 ? 32 : t <= 64 ? 64 : 128;
-  // dual = 1: the caller passes n = intermediate size of an INTERLEAVED gate/up weight, whose GEMM has 2 n / 128 tiles; that grid is
-  // sized against the three decode CTAs an SM holds (432 of 444 slots at the 14B shape, and one wave again under tensor parallelism,
-  // where the old 2-per-SM rule applied to n / 128 tiles gave 540 CTAs = two waves at TP2: csrc/trace.cuh timeline)
+  // dual = 1: the caller passes n = intermediate size of an INTERLEAVED gate/up weight, whose GEMM has 2 n / 128 tiles, counted against
+  // three slots per SM instead of two (on 132 SMs: 216 tiles at the 14B shape, split 1).  The factors fix the partial planes the reduce
+  // tails read and the fp32 order of their sum; gemm_stream_kernel deals the resulting (tile, split) units over its persistent CTAs, so
+  // they no longer have to match a number of resident CTAs.
   const long long tiles = cdiv_ll(dual ? 2 * n : n, kBM) * cdiv_ll(t, bn);
   const long long kb = cdiv_ll(k, kBK);
   const long long slots = (long long)ctx->sm_count * (bn <= 128 ? (dual && bn <= 32 ? 3 : 2) : 1);

@@ -117,6 +117,8 @@ SELECT = {
     "test_gpu_w4.py": "not (27648 or 13824 or 7168)",    # both W4A16 kernels (wgmma operand path; registers + mma.sync over the persistent schedule), small shapes
     # the FP8 decode GEMM (every code at every fragment position, partials at the small shapes) and the dequantisation kernel
     "test_gpu_fp8.py": "every_code or suggested or (partials and (704 or 1408 or 256-256 or 200 or 528)) or (dequant and 200-704)",
+    # the streaming decode GEMM against gemm_tn_kernel, bit for bit, at the small shapes (both kernels from source)
+    "test_gpu_decode_gemm.py": "bitwise_against or every_stream_shape or (split1 and not 152064) or argument_errors",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
