@@ -615,12 +615,18 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
       for (int i = 0; i < HD / 8; ++i) { oacc[i][0] *= alpha; oacc[i][1] *= alpha; }
       // ---- O += P V ; P (row g x 16 tokens) is the A operand straight from the S accumulator layout
       const uint32_t pa0 = pack2<T>(p[0][0], p[0][1]), pa2 = pack2<T>(p[1][0], p[1][1]);
+      // A token past seq_len has p = 0, but its V row holds whatever the cache held there: a row of the sequence's last page left by
+      // an earlier owner, or page 0 (another sequence's) for a page past the allocated ones.  0 * NaN = NaN, so those V elements are
+      // zeroed in the registers.  This lane's V fragments hold tokens tq*2, tq*2+1 (low, high half) of each 8-token group, as p does.
+      const uint32_t vm0 = (tok0 < seq_len ? 0x0000ffffu : 0u) | (tok0 + 1 < seq_len ? 0xffff0000u : 0u);
+      const uint32_t vm1 = (tok0 + 8 < seq_len ? 0x0000ffffu : 0u) | (tok0 + 9 < seq_len ? 0xffff0000u : 0u);
 #pragma unroll
       for (int dp = 0; dp < HD / 16; ++dp) {
         const int row = warp * 16 + (lm & 1) * 8 + lr;           // matrices: (tok0-7,dn) (tok8-15,dn) (tok0-7,dn+1) (tok8-15,dn+1)
         const int chunk = 2 * dp + (lm >> 1);
         uint32_t bf[4];
         ldsm_x4_trans(vbase + (chunk >> 3) * HALF_BYTES + row * 128 + (((chunk & 7) ^ (row & 7)) << 4), bf);
+        bf[0] &= vm0; bf[1] &= vm1; bf[2] &= vm0; bf[3] &= vm1;
         mma16816<T>(oacc[2 * dp], pa0, 0u, pa2, 0u, bf[0], bf[1]);
         mma16816<T>(oacc[2 * dp + 1], pa0, 0u, pa2, 0u, bf[2], bf[3]);
       }

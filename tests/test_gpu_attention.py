@@ -12,7 +12,7 @@ DT = torch.bfloat16
 
 
 @pytest.mark.parametrize("d", [64, 128])
-@pytest.mark.parametrize("lens", [[1], [5, 64, 65], [130, 17, 200, 1], [577]])
+@pytest.mark.parametrize("lens", [[1], [5, 64, 65], [130, 17, 200, 1], [577], [2048], [4096, 100]])
 def test_prefill_varlen_causal_gqa(d, lens):
     _prefill_case(d, lens, torch.bfloat16)
 
@@ -78,9 +78,22 @@ def test_decode_paged_fp16(d, nh, nkv, page):
     _decode_case(d, nh, nkv, page, 3, torch.float16)
 
 
-def _decode_case(d, nh, nkv, page, splits, DT):
+# long contexts: past kDecMaxPagesSm (256) page ids of one split the producer reads the page table from global memory (4200 tokens at
+# page 16, one split); 32 splits run the merge's 8-wide batches past the first with every split live.  poison: every cache row that
+# is not a live position of some sequence (rows past seq_len in a last page, the spare page of each page table, unused pages) holds
+# NaN -- the output must be the bits of the run where those rows hold zero
+@pytest.mark.parametrize("d,nh,nkv,page,splits,seq_lens,poison", [
+    (128, 40, 8, 16, 1, [4200, 17], False), (64, 4, 2, 16, 1, [4111], False), (128, 10, 2, 32, 32, [2000, 1999, 63], False),
+    (64, 4, 2, 64, 32, [2047, 5], False), (128, 10, 2, 16, 3, [1, 16, 17, 29, 333], True), (64, 4, 2, 64, 1, [1, 64, 65, 125], True),
+    (128, 40, 8, 32, 16, [70, 31, 2], True)])
+@pytest.mark.parametrize("DT", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])
+def test_decode_long_contexts_and_foreign_rows(d, nh, nkv, page, splits, seq_lens, poison, DT):
+    _decode_case(d, nh, nkv, page, splits, DT, seq_lens, poison)
+
+
+def _decode_case(d, nh, nkv, page, splits, DT, seq_lens=None, poison=False):
     c = ctx()
-    seq_lens = [1, page, page + 1, 5 * page - 3, 333][: 4 if nh == 40 else 5]
+    seq_lens = seq_lens or [1, page, page + 1, 5 * page - 3, 333][: 4 if nh == 40 else 5]
     B = len(seq_lens)
     max_pages = (max(seq_lens) + page - 1) // page + 1
     n_pages = B * max_pages + 3
@@ -91,11 +104,21 @@ def _decode_case(d, nh, nkv, page, splits, DT):
     q = torch.randn(B, nh, d, generator=g).to(DT)
     ws = torch.zeros(c.attn_decode_workspace_floats(B, nh, d, splits), device="cuda", dtype=torch.float32)
     out = torch.full((B, nh * d), float("nan"), device="cuda", dtype=DT)
-    for _ in range(2):          # twice: the arrival counters must reset themselves
+    live = torch.zeros(n_pages, page, dtype=torch.bool)
+    for b, sl in enumerate(seq_lens):
+        pos = torch.arange(sl)
+        live[perm[b, pos // page].long(), pos % page] = True
+    dead = ~live[:, None, :, None]
+    runs = [(kc.masked_fill(dead, 0), vc.masked_fill(dead, 0)), (kc.masked_fill(dead, float("nan")), vc.masked_fill(dead, float("nan")))] \
+        if poison else [(kc, vc)] * 2
+    outs = []
+    for kr, vr in runs:         # twice: the arrival counters must reset themselves
         out.fill_(float("nan"))
-        c.attn_decode(q.cuda(), kc.cuda(), vc.cuda(), perm.cuda(), torch.tensor(seq_lens, dtype=torch.int32).cuda(), B, nh, nkv, d, page,
+        c.attn_decode(q.cuda(), kr.cuda(), vr.cuda(), perm.cuda(), torch.tensor(seq_lens, dtype=torch.int32).cuda(), B, nh, nkv, d, page,
                       1.0 / math.sqrt(d), splits, ws, out)
         torch.cuda.synchronize()
+        outs.append(out.cpu().clone())
+    assert torch.equal(outs[0], outs[1])
     refs = []
     for b, sl in enumerate(seq_lens):
         pages = perm[b, : (sl + page - 1) // page].long()
@@ -104,6 +127,6 @@ def _decode_case(d, nh, nkv, page, splits, DT):
         refs.append(od.attention(q[b:b + 1].float(), kk.float(), vv.float(), nh // nkv, sl - 1))
     ref = torch.cat(refs)
     e = rel_err(out, ref)
-    record("attn_decode", d=d, nh=nh, nkv=nkv, page=page, splits=splits, err=e)
+    record("attn_decode", d=d, nh=nh, nkv=nkv, page=page, splits=splits, seq_lens=str(seq_lens), poison=int(poison), dtype=str(DT), err=e)
     assert torch.isfinite(out.float()).all()
     assert e < 1e-2

@@ -12,7 +12,7 @@ import torch
 from oracle import decoder as od
 from oracle import merge as om
 from oracle import ts_encoder as ote
-from tests.gpu_util import ctx, parity_gate, record
+from tests.gpu_util import ctx, decode_run, parity_gate, record
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -196,7 +196,7 @@ def test_fp8_model_logits_against_the_oracle_on_the_quantised_weights(dt, qwen3)
     parity_gate("fp8_next_token_logits", lg, refs[0], refs[1], dt, fixed, qwen3=int(qwen3))
     # first decode step: the token the prefill picked, through the FP8 decode GEMM
     tok = int(lg[0].float().argmax())
-    dec = _first_step_logits(model, enc)
+    dec = decode_run(model, enc, 1).logits[0, 0]
     drefs = []
     for w, st in ((same, states[0]), (f32, states[1])):
         e = w["model.embed_tokens.weight"][tok][None, :]
@@ -204,23 +204,6 @@ def test_fp8_model_logits_against_the_oracle_on_the_quantised_weights(dt, qwen3)
     # the decode GEMM multiplies by W' exactly (fp32 code * scale), the same-dtype oracle by W' rounded to the model dtype: the fixed bound
     # against that oracle gets headroom, the comparative bound against the fp32 oracle is the same as for the prefill
     parity_gate("fp8_first_decode_step_logits", dec, drefs[0][0], drefs[1][0], dt, 2e-2 if dt == torch.bfloat16 else 3e-3, qwen3=int(qwen3))
-
-
-def _first_step_logits(model, enc):
-    ids_cpu, am_cpu, counts, lay = model._prepare_inputs(enc["input_ids"], enc["attention_mask"], enc["timeseries"])
-    B = ids_cpu.shape[0]
-    pts, held = model._alloc_pages(lay.lens, 4)
-    try:
-        logits = model._prefill(lay, counts, enc["timeseries"], pts)
-        st = model._decode_state(B, 4)
-        lens32 = torch.from_numpy(lay.lens.astype(np.int32))
-        st.page_table.copy_(torch.from_numpy(pts)); st.positions.copy_(lens32 - 1); st.seq_lens.copy_(lens32); st.step_ptr.zero_()
-        model.ctx.greedy_advance(logits, B, st.out_tokens, st.step_ptr, st.cur_ids, st.positions, st.seq_lens, st.slot_map, st.page_table, model.page_size)
-        model._decode_step(st, sample=False)
-        torch.cuda.synchronize()
-        return st.full_logits[0].float().cpu().clone()
-    finally:
-        model.pool.release(held)
 
 
 def test_fp8_generate_greedy_matches_the_oracle_with_cuda_graphs():

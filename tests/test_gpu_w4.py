@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.gpu_util import ctx, record
+from tests.gpu_util import ctx, decode_run, record
 
 pytestmark = pytest.mark.gpu
 EPI_PARTIAL = 3
@@ -102,34 +102,16 @@ def test_model_decodes_through_the_packed_weights(qwen3, kernel, monkeypatch):
     l0 = model.ctx.launches
     a = model.generate(**enc, max_new_tokens=16, ignore_eos=True)
     assert model.w4 is not None and model.w4["kernel"] == kernel and model.ctx.launches > l0
-    lg4 = _first_step_logits(model, enc)
+    lg4 = decode_run(model, enc, 1).logits[0]
     w4, model.w4, model._steps = model.w4, None, {}
     b = model.generate(**enc, max_new_tokens=16, ignore_eos=True)
-    lgd = _first_step_logits(model, enc)
+    lgd = decode_run(model, enc, 1).logits[0]
     S = enc["input_ids"].shape[1]
     agree = [int(next((i for i in range(16) if a[r, S + i] != b[r, S + i]), 16)) for r in range(2)]
     err = float((lg4 - lgd).abs().max() / lgd.abs().max())
     record("w4_model_decode", qwen3=int(qwen3), kernel=kernel, greedy_agreement=str(agree), first_step_logits_rel_err=err)
     assert min(agree) >= 12          # same weights; only the K partition of the fp32 sums differs
     assert err <= 1e-2               # ... which moves a few activations by one 16-bit ulp
-
-
-def _first_step_logits(model, enc):
-    """Logits of the first decode step (the token after the prefill's) through the model's current decode path."""
-    ids_cpu, am_cpu, counts, lay = model._prepare_inputs(enc["input_ids"], enc["attention_mask"], enc["timeseries"])
-    B = ids_cpu.shape[0]
-    pts, held = model._alloc_pages(lay.lens, 4)
-    try:
-        logits = model._prefill(lay, counts, enc["timeseries"], pts)
-        st = model._decode_state(B, 4)
-        lens32 = torch.from_numpy(lay.lens.astype(np.int32))
-        st.page_table.copy_(torch.from_numpy(pts)); st.positions.copy_(lens32 - 1); st.seq_lens.copy_(lens32); st.step_ptr.zero_()
-        model.ctx.greedy_advance(logits, B, st.out_tokens, st.step_ptr, st.cur_ids, st.positions, st.seq_lens, st.slot_map, st.page_table, model.page_size)
-        model._decode_step(st, sample=False)
-        torch.cuda.synchronize()
-        return st.full_logits[:B].float().cpu().clone()
-    finally:
-        model.pool.release(held)
 
 
 def test_gptq_checkpoint_directory_decodes_through_the_packed_weights(tmp_path):

@@ -119,6 +119,11 @@ SELECT = {
     "test_gpu_fp8.py": "every_code or suggested or (partials and (704 or 1408 or 256-256 or 200 or 528)) or (dequant and 200-704)",
     # the streaming decode GEMM against gemm_tn_kernel, bit for bit, at the small shapes (both kernels from source)
     "test_gpu_decode_gemm.py": "bitwise_against or every_stream_shape or (split1 and not 152064) or argument_errors",
+    # decode parity of the tiny model (default path at batch 1 and 8, and the native step, whose projections always take the split-K
+    # partial path: logits and KV rows against the oracle, the live-slot check) and the isolation of a request from NaN in cache rows
+    # it does not own
+    "test_gpu_zz_g_decode_parity.py": "tiny-default-b1-p16 or tiny-default-b8-p32-bf16 or tiny-default-b8-p32-fp16 or tiny-native-b8-p16-bf16 "
+                                      "or (not_own and default and nan)",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
