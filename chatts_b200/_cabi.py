@@ -31,7 +31,7 @@ SYMBOLS = [
     "cts_sample_advance", "cts_rmsnorm", "cts_lm_head", "cts_decoder_step_ws_floats", "cts_decoder_step", "cts_ts_encode", "cts_gemm_decode_fused",
     "cts_peer_ll_region_bytes", "cts_peer_allreduce_ll", "cts_trace_enable", "cts_ts_encode_fused_ok", "cts_ts_encode_fused",
     "cts_rep_penalty_mark", "cts_rep_penalty_apply", "cts_gemm_w4", "cts_gemm_w4_suggest_split", "cts_gemm_w4_mma", "cts_gemm_w4_mma_suggest_split",
-    "cts_gemm_fp8", "cts_gemm_fp8_suggest_split", "cts_fp8_dequant",
+    "cts_gemm_fp8", "cts_gemm_fp8_suggest_split", "cts_fp8_dequant", "cts_attn_prefill_paged",
 ]
 FUSED_RESIDUAL, FUSED_SWIGLU, FUSED_QKV_ROPE = 0, 1, 2
 PACK_DESC_LONGS = 12
@@ -173,6 +173,8 @@ def load_library():
     lib.cts_gemm_fp8.argtypes = [vp, C.POINTER(GemmFp8Args), vp]
     lib.cts_gemm_fp8_suggest_split.argtypes = [vp, ll, ll, ll]
     lib.cts_fp8_dequant.argtypes = [vp, C.POINTER(Fp8DequantArgs), vp]
+    lib.cts_attn_prefill_paged.argtypes = [vp, vp, vp, vp, vp, vp, i, vp, i, i, i, ll, i, i, i, i, f, vp, i, vp]
+    lib.cts_attn_prefill_paged.restype = i
     lib.cts_rep_penalty_mark.argtypes = [vp, vp, vp, i, vp, i, ll, vp]
     lib.cts_rep_penalty_apply.argtypes = [vp, vp, ll, ll, i, vp, i, f, i, vp]
     lib.cts_ts_encode_fused_ok.argtypes = [C.POINTER(TsEncodeArgs)]
@@ -416,6 +418,12 @@ class Context:
     def attn_prefill(self, q, k, v, cu_seqlens, batch, max_seqlen, nh, nkv, head_dim, scale, out):
         self._chk(self.lib.cts_attn_prefill(self.h, _p(q), _p(k), _p(v), _p(cu_seqlens), batch, max_seqlen, q.shape[0], nh, nkv,
                                             head_dim, float(scale), _p(out), dtype_code(q.dtype), _stream()))
+
+    def attn_prefill_paged(self, q, cu_q, kv_lens, k_cache, v_cache, page_table, batch, max_q, nh, nkv, head_dim, page_size, scale, out):
+        """Causal attention of the packed new query rows q [total_q, nh*d] (cu_q) over each sequence's kv_lens keys in the paged cache."""
+        self._chk(self.lib.cts_attn_prefill_paged(self.h, _p(q), _p(cu_q), _p(kv_lens), _p(k_cache), _p(v_cache), k_cache.shape[0],
+                                                  _p(page_table), page_table.shape[1], batch, max_q, q.shape[0], nh, nkv, head_dim,
+                                                  page_size, float(scale), _p(out), dtype_code(q.dtype), _stream()))
 
     def attn_decode_workspace_floats(self, batch, nh, head_dim, num_splits):
         return int(self.lib.cts_attn_decode_workspace_floats(batch, nh, head_dim, num_splits))

@@ -6,6 +6,9 @@
 //                     row max / row sum, pass 2 accumulates exp(s - m) V in fragments, so no accumulator rescale
 //                     is needed; head_dim 64.  head_dim 128 runs attn_prefill_wgmma_kernel (wgmma, single-pass online
 //                     softmax with S and O in registers).
+//  cts_attn_prefill_paged : the same two kernels (a template flag) for query rows whose keys sit in the PAGED KV cache, an
+//                     already cached prefix included: query row i of sequence b is position kv_lens[b] - q_len_b + i.  Key tiles
+//                     start at position 0 whatever the prefix, so a row gets the bits it gets in a full prefill.
 //  cts_attn_decode  : one query token per sequence against the PAGED KV cache, flash-decoding split over pages.
 //                     HBM-bound (GQA intensity = nh/nkv flop/B): K/V pages are pulled with cp.async.bulk into a
 //                     double-buffered shared-memory ring (mbarrier complete_tx), all q heads of a kv head share
@@ -52,6 +55,13 @@ template <int HD> struct PfSmem {
   static constexpr size_t total = q_bytes + 4 * kv_bytes + s_bytes + p_bytes;
 };
 
+// K/V rows of a paged prefill (cts_attn_prefill_paged): where the sequence's keys come from
+struct PagedKV {
+  const int* page_table;     // [batch, max_pages]
+  const int* kv_lens;        // [batch] keys per sequence, the new rows included
+  int max_pages, page_size;
+};
+
 template <typename T, int HD>
 __device__ __forceinline__ void pf_load_tile(T* dst, const T* __restrict__ src, long long row_stride, int rows_valid) {
   // 64 rows x HD elements, 16 B per cp.async
@@ -64,11 +74,28 @@ __device__ __forceinline__ void pf_load_tile(T* dst, const T* __restrict__ src, 
   }
 }
 
+// 64 key rows kv0.. of one kv head from the paged cache [pages, nkv, page_size, HD]; rows at or past rows_valid are zero-filled
+template <typename T, int HD>
+__device__ __forceinline__ void pf_load_tile_paged(T* dst, const T* __restrict__ cache, const int* __restrict__ pt, int kv0, int rows_valid,
+                                                   int page_size, int nkv, int kvh) {
+  constexpr int LD = PfSmem<HD>::LD;
+  constexpr int CH = HD / 8;
+  for (int i = threadIdx.x; i < kPfKV * CH; i += kPfThreads) {
+    const int r = i / CH, c = i % CH;
+    const bool ok = r < rows_valid;
+    const int pos = kv0 + r;
+    const long long row = ok ? ((long long)pt[pos / page_size] * nkv + kvh) * page_size + pos % page_size : 0;
+    cp_async16(dst + r * LD + c * 8, cache + row * HD + c * 8, ok);
+  }
+}
+
 // LSE = true (the training forward, cts_attn_prefill_lse) adds one store per query row: lse[token][head] = log sum_j exp(scale s_j).
-template <typename T, int HD, bool LSE>
+// PAGED = true (cts_attn_prefill_paged): k / v are the paged cache, the query rows are the LAST len of kv_lens[b] positions.
+template <typename T, int HD, bool LSE, bool PAGED>
 __global__ void __launch_bounds__(kPfThreads)
 attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
-                    const int* __restrict__ cu_seqlens, int nh, int nkv, float scale, T* __restrict__ out, float* __restrict__ lse) {
+                    const int* __restrict__ cu_seqlens, int nh, int nkv, float scale, T* __restrict__ out, float* __restrict__ lse,
+                    PagedKV pg) {
   using SM = PfSmem<HD>;
   constexpr int LD = SM::LD, SLD = SM::SLD;
   extern __shared__ __align__(128) uint8_t pf_smem[];
@@ -81,6 +108,8 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
   pdl_wait();
   const int b = blockIdx.z, head = blockIdx.y, qt = blockIdx.x;
   const int seq0 = cu_seqlens[b], len = cu_seqlens[b + 1] - seq0;
+  const int kv_len = PAGED ? pg.kv_lens[b] : len;       // keys of the sequence; query row i sits at position off + i
+  const int off = kv_len - len;
   const int q0 = qt * kPfQ;
   if (q0 >= len) return;
   const int kvh = head / (nh / nkv);
@@ -90,15 +119,21 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
   const T* k_g = k + (long long)seq0 * kv_stride + (long long)kvh * HD;
   const T* v_g = v + (long long)seq0 * kv_stride + (long long)kvh * HD;
 
-  const int n_tiles = (min(q0 + kPfQ, len) + kPfKV - 1) / kPfKV;   // causal: kv <= last q row of this CTA
+  const int n_tiles = (min(off + q0 + kPfQ, kv_len) + kPfKV - 1) / kPfKV;   // causal: kv <= last q row of this CTA
 
   auto kbuf = [&](int st) { return kv_s + (size_t)st * 2 * kPfKV * LD; };
   auto vbuf = [&](int st) { return kv_s + (size_t)st * 2 * kPfKV * LD + (size_t)kPfKV * LD; };
   auto issue_tile = [&](int j, int st, bool with_v) {
     const int kv0 = j * kPfKV;
-    const int valid = min(kPfKV, len - kv0);
-    pf_load_tile<T, HD>(kbuf(st), k_g + (long long)kv0 * kv_stride, kv_stride, valid);
-    if (with_v) pf_load_tile<T, HD>(vbuf(st), v_g + (long long)kv0 * kv_stride, kv_stride, valid);
+    const int valid = min(kPfKV, kv_len - kv0);
+    if constexpr (PAGED) {
+      const int* pt = pg.page_table + (long long)b * pg.max_pages;
+      pf_load_tile_paged<T, HD>(kbuf(st), k, pt, kv0, valid, pg.page_size, nkv, kvh);
+      if (with_v) pf_load_tile_paged<T, HD>(vbuf(st), v, pt, kv0, valid, pg.page_size, nkv, kvh);
+    } else {
+      pf_load_tile<T, HD>(kbuf(st), k_g + (long long)kv0 * kv_stride, kv_stride, valid);
+      if (with_v) pf_load_tile<T, HD>(vbuf(st), v_g + (long long)kv0 * kv_stride, kv_stride, valid);
+    }
     cp_async_commit();
   };
 
@@ -112,6 +147,7 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
   // row statistics: lanes (2r, 2r+1) own row r of this warp's 16 rows; each covers 32 of the 64 columns
   const int r_loc = lane >> 1, c_half = lane & 1;
   const int row_g = q0 + warp * 16 + r_loc;             // query index inside the sequence
+  const int pos_g = off + row_g;                        // its key position
   float m_run = -INFINITY, l_run = 0.f;
   const float sl2 = scale * 1.4426950408889634f;        // scores are used as s * scale * log2(e) inside exp2f
 
@@ -128,7 +164,7 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
       for (int kk = 0; kk < HD / 16; ++kk) wmma::load_matrix_sync(qf[kk], q_s + (size_t)warp * 16 * LD + kk * 16, LD);
     }
     const int kv0 = j * kPfKV;
-    if (kv0 <= q0 + warp * 16 + 15) {                   // warp-uniform: tile intersects this warp's causal range
+    if (kv0 <= off + q0 + warp * 16 + 15) {             // warp-uniform: tile intersects this warp's causal range
 #pragma unroll
       for (int nt = 0; nt < kPfKV / 16; ++nt) {
         wmma::fragment<wmma::accumulator, 16, 16, 16, float> sf;
@@ -145,7 +181,7 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
       float mx = -INFINITY;
       for (int c = 0; c < 32; ++c) {
         const int col = c_half * 32 + c;
-        const float s = (kv0 + col <= row_g) ? s_w[r_loc * SLD + col] : -INFINITY;
+        const float s = (kv0 + col <= pos_g) ? s_w[r_loc * SLD + col] : -INFINITY;
         mx = fmaxf(mx, s);
       }
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
@@ -154,7 +190,7 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
       if (m_new > -INFINITY) {
         for (int c = 0; c < 32; ++c) {
           const int col = c_half * 32 + c;
-          if (kv0 + col <= row_g) sum += exp2f((s_w[r_loc * SLD + col] - m_new) * sl2);
+          if (kv0 + col <= pos_g) sum += exp2f((s_w[r_loc * SLD + col] - m_new) * sl2);
         }
       }
       sum += __shfl_xor_sync(0xffffffffu, sum, 1);
@@ -176,7 +212,7 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
     if (j + 1 < n_tiles) cp_async_wait<1>(); else cp_async_wait<0>();
     __syncthreads();
     const int kv0 = j * kPfKV;
-    if (kv0 <= q0 + warp * 16 + 15) {
+    if (kv0 <= off + q0 + warp * 16 + 15) {
 #pragma unroll
       for (int nt = 0; nt < kPfKV / 16; ++nt) {
         wmma::fragment<wmma::accumulator, 16, 16, 16, float> sf;
@@ -193,7 +229,7 @@ attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* _
       for (int c = 0; c < 32; ++c) {
         const int col = c_half * 32 + c;
         float p = 0.f;
-        if (kv0 + col <= row_g && m_run > -INFINITY) p = exp2f((s_w[r_loc * SLD + col] - m_run) * sl2);
+        if (kv0 + col <= pos_g && m_run > -INFINITY) p = exp2f((s_w[r_loc * SLD + col] - m_run) * sl2);
         p_w[r_loc * SLD + col] = DT<T>::from_f(p);
       }
       __syncwarp();
@@ -249,11 +285,13 @@ constexpr int kWgHalf = 64 * 128;                         // one [64 rows x 128 
 constexpr int kWgStageBytes = 4 * kWgHalf;                // K and V tile
 constexpr int kWgSmem = 2 * kWgHalf + kWgStages * kWgStageBytes;
 
-template <typename T, bool LSE>
+// PAGED = true (cts_attn_prefill_paged): tm_k / tm_v map the paged cache as [pages * nkv * page_size rows, 128] with page_size-row
+// boxes; a 64-key stage is filled by 64 / page_size boxes per 64-column half, which lands the same swizzled tile as one 64-row box.
+template <typename T, bool LSE, bool PAGED>
 __global__ void __launch_bounds__(kWgThreads, 2)
 attn_prefill_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                           const __grid_constant__ CUtensorMap tm_v, const int* __restrict__ cu_seqlens, int nh, int nkv, float scale,
-                          T* __restrict__ out, float* __restrict__ lse) {
+                          T* __restrict__ out, float* __restrict__ lse, PagedKV pg) {
   extern __shared__ uint8_t wg_raw[];
   __shared__ uint64_t q_bar, full_bar[kWgStages], empty_bar[kWgStages];
   constexpr bool kIsBf16 = std::is_same<T, __nv_bfloat16>::value;
@@ -275,9 +313,11 @@ attn_prefill_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid
   __syncthreads();
   pdl_wait();                                            // Q / K / V / cu_seqlens come from the predecessors
   const int seq0 = cu_seqlens[b], len = cu_seqlens[b + 1] - seq0;
+  const int kv_len = PAGED ? pg.kv_lens[b] : len;        // keys of the sequence; query row i sits at position off + i
+  const int off = kv_len - len;
   const int q0 = qt * kWgQ;
   if (q0 >= len) return;                                 // CTA-uniform; nothing was issued yet
-  const int kv_end = min(len, q0 + kWgQ);                // causal: keys 0 .. q0 + 63
+  const int kv_end = min(kv_len, off + q0 + kWgQ);       // causal: keys 0 .. off + q0 + 63
   const int ntiles = (kv_end + kWgKV - 1) / kWgKV;
 
   if (warp == 4) {
@@ -286,16 +326,35 @@ attn_prefill_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid
       mbar_expect_tx(&q_bar, 2u * kWgHalf);
       tma_load_2d(q_s, &tm_q, &q_bar, head * 128, seq0 + q0, CTS_L2_EVICT_FIRST);
       tma_load_2d(q_s + kWgHalf, &tm_q, &q_bar, head * 128 + 64, seq0 + q0, CTS_L2_EVICT_FIRST);
+      const int npp = PAGED ? kWgKV / pg.page_size : 1;  // pages per 64-key stage
       for (int j = 0; j < ntiles; ++j) {
         const int s = j % kWgStages;
+        int pid[4] = {0, 0, 0, 0};
+        if constexpr (PAGED) {                           // page ids read before the wait: the L2 round trip overlaps it
+#pragma unroll
+          for (int p = 0; p < 4; ++p)
+            if (p < npp) pid[p] = pg.page_table[(long long)b * pg.max_pages + min(j * npp + p, pg.max_pages - 1)];
+        }
         mbar_wait(&empty_bar[s], ((uint32_t)(j / kWgStages) & 1u) ^ 1u);
         mbar_expect_tx(&full_bar[s], (uint32_t)kWgStageBytes);
         uint8_t* st = kv_s + (size_t)s * kWgStageBytes;
-        const int row = seq0 + j * kWgKV;
-        tma_load_2d(st, &tm_k, &full_bar[s], kvh * 128, row, CTS_L2_EVICT_LAST);
-        tma_load_2d(st + kWgHalf, &tm_k, &full_bar[s], kvh * 128 + 64, row, CTS_L2_EVICT_LAST);
-        tma_load_2d(st + 2 * kWgHalf, &tm_v, &full_bar[s], kvh * 128, row, CTS_L2_EVICT_LAST);
-        tma_load_2d(st + 3 * kWgHalf, &tm_v, &full_bar[s], kvh * 128 + 64, row, CTS_L2_EVICT_LAST);
+        if constexpr (PAGED) {
+#pragma unroll
+          for (int p = 0; p < 4; ++p) {
+            if (p >= npp) break;
+            const int row0 = (pid[p] * nkv + kvh) * pg.page_size, o = p * pg.page_size * 128;
+            tma_load_2d(st + o, &tm_k, &full_bar[s], 0, row0, CTS_L2_EVICT_LAST);
+            tma_load_2d(st + kWgHalf + o, &tm_k, &full_bar[s], 64, row0, CTS_L2_EVICT_LAST);
+            tma_load_2d(st + 2 * kWgHalf + o, &tm_v, &full_bar[s], 0, row0, CTS_L2_EVICT_LAST);
+            tma_load_2d(st + 3 * kWgHalf + o, &tm_v, &full_bar[s], 64, row0, CTS_L2_EVICT_LAST);
+          }
+        } else {
+          const int row = seq0 + j * kWgKV;
+          tma_load_2d(st, &tm_k, &full_bar[s], kvh * 128, row, CTS_L2_EVICT_LAST);
+          tma_load_2d(st + kWgHalf, &tm_k, &full_bar[s], kvh * 128 + 64, row, CTS_L2_EVICT_LAST);
+          tma_load_2d(st + 2 * kWgHalf, &tm_v, &full_bar[s], kvh * 128, row, CTS_L2_EVICT_LAST);
+          tma_load_2d(st + 3 * kWgHalf, &tm_v, &full_bar[s], kvh * 128 + 64, row, CTS_L2_EVICT_LAST);
+        }
       }
     }
     return;
@@ -314,6 +373,20 @@ attn_prefill_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid
   for (int j = 0; j < ntiles; ++j) {
     const int s = j % kWgStages;
     mbar_wait(&full_bar[s], (uint32_t)(j / kWgStages) & 1u);
+    if constexpr (PAGED) {
+      // Keys at or past kv_len get p = 0, but their V rows hold whatever the cache holds there (recycled pages are never cleared,
+      // page-table entries past the sequence point anywhere) and 0 * NaN = NaN: those rows are zeroed before the P V MMA.
+      const int nz = (j + 1) * kWgKV - kv_len;           // CTA-uniform
+      if (nz > 0) {
+        uint8_t* vs = kv_s + (size_t)s * kWgStageBytes + 2 * kWgHalf;
+        for (int i = threadIdx.x; i < nz * 16; i += 128) {  // 16-byte chunks: 8 per 128-byte row of each half (the swizzle stays in the row)
+          const int r = kWgKV - nz + (i >> 4), c = i & 15;
+          *reinterpret_cast<uint4*>(vs + (c >> 3) * kWgHalf + r * 128 + (c & 7) * 16) = make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async_smem();                        // generic-proxy writes -> visible to the tensor core
+        named_bar_sync(1, 128);
+      }
+    }
     const uint32_t k_addr = smem_u32(kv_s + (size_t)s * kWgStageBytes), v_addr = k_addr + 2 * kWgHalf;
     float sc[32];
 #pragma unroll
@@ -335,7 +408,7 @@ attn_prefill_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int h = (i >> 1) & 1, row = h ? r1 : r0, col = j * kWgKV + acc_col(i);
-      const float v = (col > row || col >= len) ? -INFINITY : sc[i] * sl2;
+      const float v = (col > off + row || col >= kv_len) ? -INFINITY : sc[i] * sl2;
       sc[i] = v;
       mx[h] = fmaxf(mx[h], v);
     }
@@ -747,9 +820,10 @@ static int attn_prefill_impl(cts_ctx* ctx, const void* q, const void* k, const v
     const size_t smem_w = (size_t)kWgSmem + 1024;
 #define WG_LAUNCH(TT, LSEV)                                                                                  \
   {                                                                                                          \
-    auto kern = attn_prefill_wgmma_kernel<TT, LSEV>;                                                         \
+    auto kern = attn_prefill_wgmma_kernel<TT, LSEV, false>;                                                  \
     CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));     \
-    CTS_CUDA(ctx, launch_pdl(kern, gw, dim3(kWgThreads), smem_w, st, 1, tm_q, tm_k, tm_v, cu_seqlens, nh, nkv, scale, (TT*)out, lse)); \
+    CTS_CUDA(ctx, launch_pdl(kern, gw, dim3(kWgThreads), smem_w, st, 1, tm_q, tm_k, tm_v, cu_seqlens, nh, nkv, scale, (TT*)out, lse, \
+                             PagedKV{}));                                                                   \
   }
     if (dtype == CTS_BF16) {
       if (lse) WG_LAUNCH(__nv_bfloat16, true) else WG_LAUNCH(__nv_bfloat16, false)
@@ -762,11 +836,11 @@ static int attn_prefill_impl(cts_ctx* ctx, const void* q, const void* k, const v
   dim3 grid((unsigned)((max_seqlen + kPfQ - 1) / kPfQ), (unsigned)nh, (unsigned)batch);
 #define PF_LAUNCH2(TT, HDV, LSEV)                                                                            \
   {                                                                                                          \
-    auto kern = attn_prefill_kernel<TT, HDV, LSEV>;                                                          \
+    auto kern = attn_prefill_kernel<TT, HDV, LSEV, false>;                                                   \
     const size_t smem = PfSmem<HDV>::total;                                                                  \
     CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));       \
     CTS_CUDA(ctx, launch_pdl(kern, grid, dim3(kPfThreads), smem, st, 1, (const TT*)q, (const TT*)k, (const TT*)v, cu_seqlens, nh, nkv, \
-                             scale, (TT*)out, lse));                                                         \
+                             scale, (TT*)out, lse, PagedKV{}));                                              \
   }
 #define PF_LAUNCH(TT, HDV) { if (lse) PF_LAUNCH2(TT, HDV, true) else PF_LAUNCH2(TT, HDV, false) }
   if (dtype == CTS_BF16) {
@@ -795,6 +869,61 @@ extern "C" int cts_attn_prefill_lse(cts_ctx* ctx, const void* q, const void* k, 
   CTS_CHECK_ARG(ctx, lse != nullptr, "null lse");
   return attn_prefill_impl(ctx, q, k, v, cu_seqlens, batch, max_seqlen, total_tokens_hint, nh, nkv, head_dim, scale, out, lse, dtype,
                            stream);
+}
+
+extern "C" int cts_attn_prefill_paged(cts_ctx* ctx, const void* q, const int* cu_q, const int* kv_lens, const void* k_cache,
+                                      const void* v_cache, int num_pages, const int* page_table, int max_pages, int batch, int max_q,
+                                      long long total_q, int nh, int nkv, int head_dim, int page_size, float scale, void* out, int dtype,
+                                      void* stream) {
+  if (!ctx) return CTS_ERR_BAD_ARG;
+  CTS_CHECK_ARG(ctx, q && cu_q && kv_lens && k_cache && v_cache && page_table && out, "null pointer");
+  CTS_CHECK_ARG(ctx, nh > 0 && nkv > 0 && nh % nkv == 0 && nh / nkv <= kMaxGroup, "nh/nkv must be an integer <= 8");
+  CTS_CHECK_ARG(ctx, page_size == 16 || page_size == 32 || page_size == 64, "page_size must be 16, 32 or 64");
+  CTS_CHECK_ARG(ctx, num_pages > 0 && max_pages > 0, "num_pages / max_pages");
+  CTS_CHECK_ARG(ctx, (long long)num_pages * nkv * page_size < 2147483647LL, "KV cache too large for 32-bit TMA row coordinates");
+  CTS_CHECK_ARG(ctx, batch >= 0 && max_q >= 0 && total_q >= 0, "batch / max_q / total_q");
+  CTS_CHECK_ARG(ctx, dtype == CTS_BF16 || dtype == CTS_F16, "dtype");
+  if (head_dim != 64 && head_dim != 128)
+    return cts_set_error(ctx, CTS_ERR_UNSUPPORTED, "cts_attn_prefill_paged: head_dim %d (64 or 128)", head_dim);
+  if (batch == 0 || max_q == 0) return CTS_OK;
+  CTS_CHECK_ARG(ctx, total_q > 0 && batch <= 65535 && nh <= 65535, "grid");
+  cudaStream_t st = (cudaStream_t)stream;
+  const PagedKV pg{page_table, kv_lens, max_pages, page_size};
+  if (head_dim == 128) {
+    const long long rows = (long long)num_pages * nkv * page_size;
+    CUtensorMap tm_q, tm_k, tm_v;
+    int rc = cts_make_tmap_2d(ctx, &tm_q, q, total_q, (long long)nh * 128, (long long)nh * 128, kWgQ, dtype == CTS_BF16);
+    if (rc) return rc;
+    rc = cts_make_tmap_2d(ctx, &tm_k, k_cache, rows, 128, 128, page_size, dtype == CTS_BF16);
+    if (rc) return rc;
+    rc = cts_make_tmap_2d(ctx, &tm_v, v_cache, rows, 128, 128, page_size, dtype == CTS_BF16);
+    if (rc) return rc;
+    dim3 gw((unsigned)((max_q + kWgQ - 1) / kWgQ), (unsigned)nh, (unsigned)batch);
+    const size_t smem_w = (size_t)kWgSmem + 1024;
+#define WGP_LAUNCH(TT)                                                                                       \
+  {                                                                                                          \
+    auto kern = attn_prefill_wgmma_kernel<TT, false, true>;                                                  \
+    CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));     \
+    CTS_CUDA(ctx, launch_pdl(kern, gw, dim3(kWgThreads), smem_w, st, 1, tm_q, tm_k, tm_v, cu_q, nh, nkv, scale, (TT*)out,     \
+                             (float*)nullptr, pg));                                                         \
+  }
+    if (dtype == CTS_BF16) WGP_LAUNCH(__nv_bfloat16) else WGP_LAUNCH(__half)
+#undef WGP_LAUNCH
+    return CTS_OK;
+  }
+  dim3 grid((unsigned)((max_q + kPfQ - 1) / kPfQ), (unsigned)nh, (unsigned)batch);
+#define PFP_LAUNCH(TT)                                                                                       \
+  {                                                                                                          \
+    auto kern = attn_prefill_kernel<TT, 64, false, true>;                                                    \
+    const size_t smem = PfSmem<64>::total;                                                                   \
+    CTS_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));       \
+    CTS_CUDA(ctx, launch_pdl(kern, grid, dim3(kPfThreads), smem, st, 1, (const TT*)q, (const TT*)k_cache, (const TT*)v_cache, cu_q, \
+                             nh, nkv, scale, (TT*)out, (float*)nullptr, pg));                                \
+  }
+  if (dtype == CTS_BF16) PFP_LAUNCH(__nv_bfloat16) else PFP_LAUNCH(__half)
+#undef PFP_LAUNCH
+  CTS_LAUNCH_CHECK(ctx);
+  return CTS_OK;
 }
 
 extern "C" long long cts_attn_decode_workspace_floats(int batch, int nh, int head_dim, int num_splits) {

@@ -35,6 +35,7 @@ class Request:
     pages: list = field(default_factory=list)
     done: bool = False
     error: Exception = None            # set when the request could not be admitted (over-long, or larger than the whole KV pool)
+    cached_positions: int = 0          # prompt positions whose KV came from the prefix cache (model built with enable_prefix_caching)
 
 
 class ContinuousEngine:
@@ -126,7 +127,7 @@ class ContinuousEngine:
                 ts = None
             try:
                 _, _, counts, lay = m._prepare_inputs(ids, am, ts)
-                pts, held = m._alloc_pages(lay.lens, max(r.max_new_tokens for r in group) + self.k)
+                pts, held, keys, cached = m._alloc_prompt(lay, ts, max(r.max_new_tokens for r in group) + self.k)
             except RuntimeError as e:                      # KV cache full (_alloc_pages takes nothing when it fails)
                 if self.active:                            # pages will come back: put the group back and wait for a release
                     for r in reversed(group):
@@ -156,7 +157,8 @@ class ContinuousEngine:
                         self.max_prefill = saved
                     free = self._free_slots()
                 continue
-            logits = m._prefill(lay, counts, ts, pts)
+            logits = m._prefill(lay, counts, ts, pts, cached=cached)
+            m._prefix_register(keys, pts, lay.lens, cached)
             # first token + advanced per-sequence state through the greedy kernel on a group-sized scratch state
             g = len(group)
             dev = m.device
@@ -177,6 +179,7 @@ class ContinuousEngine:
                 need = (int(lay.lens[i]) + max(q.max_new_tokens for q in group) + self.k + m.page_size - 1) // m.page_size
                 r.pages = [int(x) for x in pts[i, :need]]
                 r.slot = free[i]
+                r.cached_positions = int(cached[i]) if cached is not None else 0
                 r.tokens.append(int(first[i]))
                 self.active[r.slot] = r
                 self._check_done(r)

@@ -17,7 +17,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from . import _cabi, layout
+from . import _cabi, layout, prefix_cache
 from .trace import span
 from ._cabi import EPI_NONE, EPI_PARTIAL_F32, EPI_RESIDUAL, EPI_SWIGLU_IL
 from .config import ChatTSConfig
@@ -56,6 +56,9 @@ class PagePool:
     def release(self, pages):
         self.free.extend(reversed(pages))
 
+    def available(self):
+        return len(self.free)
+
 
 def _check_quantization(quantization):
     if quantization not in (None, "fp8"):
@@ -70,7 +73,10 @@ class _Step:
 class ChatTSForCausalLM:
     def __init__(self, config, state_dict, device="cuda", dtype=torch.bfloat16, tp_rank=0, tp_size=1,
                  max_batch=32, max_seq_len=2048, page_size=64, use_cuda_graph=True, comm=None,
-                 use_peer_allreduce=True, graph_with_tp=True, use_chain=None, use_sample_kernel=None, use_native_step=None, use_fused_decode=None, use_peer_ll=None):
+                 use_peer_allreduce=True, graph_with_tp=True, use_chain=None, use_sample_kernel=None, use_native_step=None, use_fused_decode=None, use_peer_ll=None,
+                 enable_prefix_caching=False):
+        if enable_prefix_caching and tp_size > 1:
+            raise ValueError("enable_prefix_caching is single-GPU only (tensor_parallel_size must be 1)")
         if not torch.cuda.is_available():
             raise _cabi.CtsError("chatts_b200 needs an H100 (sm_90a) GPU; there is no CPU fallback")
         self.config, self.dtype = config, dtype
@@ -128,7 +134,12 @@ class ChatTSForCausalLM:
         self.n_pos = n_pos
         num_pages = max_batch * self.max_pages
         self.kv = torch.zeros(self.L, 2, num_pages, self.nkv, page_size, self.d, device=self.device, dtype=dtype)
-        self.pool = PagePool(num_pages)
+        # prefix caching (chatts_b200/prefix_cache.py): generate() and ContinuousEngine reuse the KV pages of a prompt prefix an earlier
+        # prefill wrote; forward() never does.  Off: the plain free list, and every prefill computes every position.
+        self.enable_prefix_caching = bool(enable_prefix_caching)
+        self.pool = prefix_cache.CachingPagePool(num_pages) if self.enable_prefix_caching else PagePool(num_pages)
+        self._prefix_epoch = 0
+        self._prefix_queried = self._prefix_hits = 0
         self._steps = {}
         self.peer, self.peer_tokens = None, 0
         if tp_size > 1 and use_peer_allreduce:
@@ -240,6 +251,7 @@ class ChatTSForCausalLM:
         if self.fp8 is not None:
             raise ValueError("merge_lora on an FP8 model: the 16-bit projection weights are gone -- merge the adapter into the 16-bit "
                              "model first, then call quantize_fp8()")
+        self._prefix_clear()
         if isinstance(adapter, str):
             cfg_path = os.path.join(adapter, "adapter_config.json")
             if os.path.exists(cfg_path):
@@ -303,6 +315,7 @@ class ChatTSForCausalLM:
             raise ValueError("attach_w4 on an FP8 model: the projections are already quantised")
         if self.tp_size != 1:
             raise ValueError("W4A16 decode weights are single-GPU (tensor parallelism uses the dequantised weights)")
+        self._prefix_clear()
         dev = self.device
         gs = int(group_size)
         w4 = dict(group_size=gs, qkv=[], o=[], gu=[], d=[])
@@ -352,6 +365,7 @@ class ChatTSForCausalLM:
         from .weights import dequantize_w4, W4_NIBBLE_OF_K  # noqa: F401
         if self.fp8 is not None:
             raise ValueError("quantize_w4_synthetic on an FP8 model: the projections are already quantised")
+        self._prefix_clear()
         g = torch.Generator(device=self.device).manual_seed(seed)
         packed = {}
 
@@ -418,6 +432,7 @@ class ChatTSForCausalLM:
         # dequantisation overwrites it)
         fp8["scratch"] = torch.empty(biggest, device=self.device, dtype=self.dtype)
         self.fp8 = fp8
+        self._prefix_clear()
         self._steps = {}
         if hasattr(self, "_layer_list"):
             del self._layer_list
@@ -703,16 +718,23 @@ class ChatTSForCausalLM:
             self._host_counts = (host[0], host[1])
             cnt_h = host[1].numpy().astype(np.int64)
         if layout_kind == "hf":
-            import os as _os
-            mode = _os.environ.get("CTS_TS_MERGE_MODE") or getattr(cfg, "ts_merge_mode", "insert")
-            lay = layout.hf_layout(ids_cpu, am_cpu, cnt_h, cfg.ts_token_start_index, mode)
+            lay = layout.hf_layout(ids_cpu, am_cpu, cnt_h, cfg.ts_token_start_index, self._merge_mode())
         else:
             lay = layout.vllm_layout(ids_cpu, int(cnt_h.sum()), cfg.ts_token_start_index)
         return ids_cpu, am_cpu, counts, lay
 
-    def _prefill(self, lay, counts, timeseries, page_tables, all_logits=False):
+    def _merge_mode(self):
+        import os as _os
+        return _os.environ.get("CTS_TS_MERGE_MODE") or getattr(self.config, "ts_merge_mode", "insert")
+
+    def _prefill(self, lay, counts, timeseries, page_tables, all_logits=False, cached=None):
         """Runs the prompt through the TS encoder + decoder, fills the paged KV cache, returns logits
-        ([B,V] last position, or [T,V] for every merged position when all_logits)."""
+        ([B,V] last position, or [T,V] for every merged position when all_logits).  ``cached`` (prefix caching, from _alloc_prompt):
+        per sequence, the number of leading positions whose KV the pages of ``page_tables`` already hold; only the rest is computed."""
+        if cached is not None and int(np.max(cached, initial=0)) > 0:
+            if all_logits:
+                raise ValueError("all_logits needs every position computed: no prefix-cache hits")
+            return self._prefill_suffix(lay, counts, timeseries, page_tables, np.asarray(cached, dtype=np.int64))
         c, dev, dt = self.ctx, self.device, self.dtype
         T, B = lay.total, lay.cu_seqlens.shape[0] - 1
         lens = lay.lens
@@ -747,6 +769,116 @@ class ChatTSForCausalLM:
         c.gemm(hn, self.lm_head, logits, epilogue=EPI_NONE)
         return self._gather_vocab(logits)
 
+    def _prefill_suffix(self, lay, counts, timeseries, page_tables, cached):
+        """_prefill of the positions past each sequence's cached prefix: the embeddings, the series that have a patch row among them and
+        the decoder layers run on those positions only, and attention reads the cached keys from the pages (cts_attn_prefill_paged)."""
+        c, dev, dt = self.ctx, self.device, self.dtype
+        B, lens, cu = lay.cu_seqlens.shape[0] - 1, lay.lens.astype(np.int64), lay.cu_seqlens.astype(np.int64)
+        if int(lens.max()) > self.n_pos:
+            raise ValueError(f"prompt of {int(lens.max())} positions exceeds max_seq_len {self.n_pos}")
+        qlens = lens - cached
+        sel = np.concatenate([np.arange(cu[b] + cached[b], cu[b + 1]) for b in range(B)])      # merged positions computed now
+        T = int(sel.shape[0])
+        row_of = np.full(lay.total, T, dtype=np.int64)        # merged position -> row of this call; T: the discard row
+        row_of[sel] = np.arange(T)
+        st = self._alloc_step(T, decode=False)
+        st.h = torch.empty(T + 1, self.H, device=dev, dtype=dt)
+        pos = lay.positions[sel].astype(np.int64)
+        b_of = np.repeat(np.arange(B), qlens)
+        slot = page_tables[b_of, pos // self.page_size].astype(np.int64) * self.page_size + pos % self.page_size
+        cu_q = np.concatenate([[0], np.cumsum(qlens)])
+        host = np.concatenate([lay.ids[sel], pos, slot, cu_q, lens, page_tables.reshape(-1)]).astype(np.int32)
+        dbuf = torch.from_numpy(host).pin_memory().to(dev, non_blocking=True)
+        ids_d, st.positions, st.slot_map = dbuf[:T], dbuf[T:2 * T], dbuf[2 * T:3 * T]
+        cu_d, kvl_d = dbuf[3 * T:3 * T + B + 1], dbuf[3 * T + B + 1:3 * T + 2 * B + 1]
+        pt_d = dbuf[3 * T + 2 * B + 1:].view(B, -1)
+        c.embed_gather(self.embed, ids_d, st.h, t=T)
+        if counts is not None and lay.row_map.shape[0] > 0:
+            # a series is encoded when one of its patch rows is computed now (whole: the rows of a series that straddles the cached
+            # boundary land in the discard row); a series entirely inside the cached prefix is not encoded at all
+            cnt = self._host_counts[1].numpy().astype(np.int64)
+            series = np.repeat(np.arange(cnt.shape[0]), cnt)
+            rows = row_of[lay.row_map]
+            keep = np.bincount(series[rows < T], minlength=cnt.shape[0]) > 0
+            if keep.any():
+                rmap = torch.from_numpy(rows[keep[series]].astype(np.int32)).to(dev, non_blocking=True)
+                if keep.all():
+                    sub, sub_counts, host_counts = timeseries, counts, self._host_counts
+                else:
+                    idx = np.nonzero(keep)[0]
+                    sub = counts[0][torch.from_numpy(idx).to(counts[0].device)]
+                    sub_counts = self.ts_encoder.patch_counts(sub)
+                    host_counts = tuple(h[torch.from_numpy(idx)] for h in self._host_counts)
+                self.ts_encoder.encode(sub, out=st.h, row_map=rmap, counts=sub_counts, host_counts=host_counts)
+        max_q, scale = int(qlens.max()), 1.0 / math.sqrt(self.d)
+
+        def attend(l):
+            c.attn_prefill_paged(st.q, cu_d, kvl_d, self.kv[l, 0], self.kv[l, 1], pt_d, B, max_q, self.nh, self.nkv, self.d,
+                                 self.page_size, scale, st.ao)
+
+        self._layers(st, T, attend)
+        last = torch.from_numpy(cu_q[1:] - 1).to(dev)
+        hn = st.xn.index_select(0, last).contiguous()
+        logits = torch.empty(B, self.V, device=dev, dtype=dt)
+        c.gemm(hn, self.lm_head, logits, epilogue=EPI_NONE)
+        return logits
+
+    # ------------------------------------------------------------------------------------------ prefix caching
+    def _prefix_clear(self):
+        """Invalidation: every weight change bumps the epoch of the key chain and drops the index (pages still in use stay with their
+        holders as private pages)."""
+        self._prefix_epoch += 1
+        if self.enable_prefix_caching:
+            self.pool.clear()
+
+    def prefix_cache_stats(self):
+        """Prompt positions prefilled through the cache so far, how many of them were hits, the pages in the index, pages evicted."""
+        pool = self.pool
+        return dict(queried_positions=self._prefix_queried, hit_positions=self._prefix_hits,
+                    cached_pages=len(pool.page_of) if self.enable_prefix_caching else 0,
+                    evictions=pool.evictions if self.enable_prefix_caching else 0)
+
+    def _alloc_prompt(self, lay, timeseries, extra):
+        """Pages for the prompts of ``lay`` plus ``extra`` decode positions each: (page_tables, held, keys, cached).  With prefix
+        caching on, the leading full pages an earlier prefill indexed are shared (cached = positions per sequence they hold) and keys
+        are what _prefix_register indexes once the prefill is enqueued; off, keys and cached are None."""
+        if not self.enable_prefix_caching:
+            return self._alloc_pages(lay.lens, extra) + (None, None)
+        cnt = self._host_counts[1].numpy() if lay.row_map.shape[0] > 0 else np.zeros(0, dtype=np.int64)
+        seed = prefix_cache.chain_seed(self._merge_mode(), self.page_size, self._prefix_epoch)
+        keys = prefix_cache.page_keys(lay, prefix_cache.series_digests(timeseries) if cnt.shape[0] else [], cnt, seed, self.page_size)
+        needs = self._page_needs(lay.lens, extra)
+        pool, ps = self.pool, self.page_size
+        hits = [pool.lookup(keys[b][: (int(n) - 1) // ps]) for b, n in enumerate(lay.lens)]
+        hit_set = {p for h in hits for p in h}
+        new = sum(n - len(h) for n, h in zip(needs, hits))
+        # all-or-nothing: hits + free + evictable (minus the evictable pages this batch hits) against the need, before any reference
+        avail = len(pool.free) + sum(1 for p in pool.evictable if p not in hit_set)
+        if new > avail:
+            raise RuntimeError(f"KV cache exhausted: need {new} new pages, {avail} free or evictable of {pool.num_pages}")
+        for h in hits:
+            pool.acquire(h)
+        pt = np.zeros((len(needs), self.max_pages), dtype=np.int32)
+        held = []
+        for b, (n, h) in enumerate(zip(needs, hits)):
+            pages = h + pool.alloc(n - len(h))
+            pt[b, :n] = pages
+            held += pages
+        cached = np.array([len(h) * ps for h in hits], dtype=np.int64)
+        self._prefix_queried += int(lay.lens.sum())
+        self._prefix_hits += int(cached.sum())
+        return pt, held, keys, cached
+
+    def _prefix_register(self, keys, page_tables, lens, cached):
+        """Indexes the full prompt pages a prefill has just been enqueued to write (later prefills on the stream are ordered after it,
+        and prompt pages are never written again).  No-op when prefix caching is off."""
+        if keys is None:
+            return
+        ps = self.page_size
+        for b, ks in enumerate(keys):
+            for k in range(int(cached[b]) // ps, min(len(ks), int(lens[b]) // ps)):
+                self.pool.register(ks[k], int(page_tables[b, k]))
+
     def _gather_vocab(self, logits):
         if self.tp_size == 1:
             return logits
@@ -772,13 +904,10 @@ class ChatTSForCausalLM:
 
     __call__ = forward
 
-    def _alloc_pages(self, lens, extra):
+    def _page_needs(self, lens, extra):
         B = len(lens)
         if B > self.max_batch:
             raise ValueError(f"batch {B} exceeds max_batch {self.max_batch}")
-        pt = np.zeros((B, self.max_pages), dtype=np.int32)
-        # all-or-nothing: every need is checked before the first page leaves the pool, so a failure can never strand pages
-        # (ContinuousEngine._admit retries a RuntimeError; a leak there would shrink the pool for good)
         needs = []
         for b in range(B):
             n_tok = int(lens[b]) + extra
@@ -789,8 +918,15 @@ class ChatTSForCausalLM:
             if need > self.max_pages:
                 raise ValueError(f"sequence of {n_tok} tokens exceeds max_seq_len {self.max_seq_len}")
             needs.append(need)
-        if sum(needs) > len(self.pool.free):
-            raise RuntimeError(f"KV cache exhausted: need {sum(needs)} pages, {len(self.pool.free)} free of {self.pool.num_pages}")
+        return needs
+
+    def _alloc_pages(self, lens, extra):
+        needs = self._page_needs(lens, extra)
+        pt = np.zeros((len(needs), self.max_pages), dtype=np.int32)
+        # all-or-nothing: every need is checked before the first page leaves the pool, so a failure can never strand pages
+        # (ContinuousEngine._admit retries a RuntimeError; a leak there would shrink the pool for good)
+        if sum(needs) > self.pool.available():
+            raise RuntimeError(f"KV cache exhausted: need {sum(needs)} pages, {self.pool.available()} free of {self.pool.num_pages}")
         held = []
         try:
             for b, need in enumerate(needs):
@@ -972,10 +1108,12 @@ class ChatTSForCausalLM:
                 box = [seed]
                 torch.distributed.broadcast_object_list(box, src=0, group=self.comm)
                 seed = int(box[0])
-        page_tables, held = self._alloc_pages(lay.lens, max_new_tokens)
+        page_tables, held, keys, cached = self._alloc_prompt(lay, timeseries, max_new_tokens)
         try:
             with span("cts.prefill"):
-                logits = self._prefill(lay, counts, timeseries, page_tables)
+                logits = self._prefill(lay, counts, timeseries, page_tables, cached=cached)
+            self._prefix_register(keys, page_tables, lay.lens, cached)
+            self.last_cached_positions = cached          # per row: prompt positions whose KV came from the prefix cache (None: caching off)
             st = self._decode_state(B, max_new_tokens)
             lens32 = torch.from_numpy(lay.lens.astype(np.int32))
             st.page_table.copy_(torch.from_numpy(page_tables), non_blocking=True)

@@ -364,6 +364,8 @@ def parse_args(argv=None):
     ap.add_argument("--steps-per-round", type=int, default=4, help="continuous scheduler: decode steps between two host reads")
     ap.add_argument("--quantization", default=None, choices=["fp8"],
                     help="fp8: decoder projections quantised to FP8 (e4m3, per-output-channel scales) at load time")
+    ap.add_argument("--enable-prefix-caching", action="store_true",
+                    help="reuse the KV pages of a prompt prefix (series included) an earlier request wrote; single GPU")
     return ap.parse_args(argv)
 
 
@@ -377,7 +379,7 @@ def main():
         from transformers import AutoTokenizer
         tok = AutoTokenizer.from_pretrained(args.model, trust_remote_code=True)
     llm = LLM(model=args.model, tokenizer=tok, dtype=args.dtype, max_model_len=args.max_model_len, max_num_seqs=args.max_num_seqs,
-              limit_mm_per_prompt={"timeseries": limit}, quantization=args.quantization)
+              limit_mm_per_prompt={"timeseries": limit}, quantization=args.quantization, enable_prefix_caching=args.enable_prefix_caching)
     uvicorn.run(create_app(llm, args.served_model_name, args.batch_window_ms, limit, args.scheduler, args.steps_per_round),
                 host=args.host, port=args.port)
 

@@ -102,6 +102,7 @@ class IncrementalDecoder:
 class RequestOutput:
     prompt: str
     outputs: list
+    num_cached_tokens: int = 0          # prompt positions (patch rows included) whose KV came from the prefix cache
 
 
 def _free_port():
@@ -141,7 +142,7 @@ def _make_llm(**kw):
 class LLM:
     def __init__(self, model=None, tokenizer=None, config=None, state_dict=None, tensor_parallel_size=1, dtype="bfloat16",
                  max_model_len=2048, max_num_seqs=32, limit_mm_per_prompt=None, trust_remote_code=True, seed=1234,
-                 distributed_backend="nccl", quantization=None, **kw):
+                 distributed_backend="nccl", quantization=None, enable_prefix_caching=False, **kw):
         """tensor_parallel_size = k > 1 (every caller of the reference passes it: demo/demo_vllm.py:30, llm_utils.py:153-154):
           * under torchrun / an initialised process group of k ranks the engine ATTACHES: every rank constructs the LLM and makes the
             same generate() calls (rank r holds shard r);
@@ -149,12 +150,18 @@ class LLM:
             README.md:141) that build their shards and mirror every generate() call of this process (rank 0) -- the model must then
             be named by a path or by config + seed (a ChatTSForCausalLM instance cannot be sent to another process).
         quantization: None (the checkpoint's 16-bit weights) or "fp8" (vLLM's weight-only FP8: ChatTSForCausalLM.quantize_fp8 at load time,
-        on every rank)."""
+        on every rank).
+        enable_prefix_caching: the KV pages of a prompt prefix an earlier request wrote are reused, series included (prefix_cache.py);
+        single GPU only."""
         import os
         if quantization not in (None, "fp8"):
             raise ValueError(f"quantization={quantization!r}: supported are None and 'fp8'")
-        self._tp_procs, self._tp_driver = [], False
         tp = int(tensor_parallel_size or 1)
+        if enable_prefix_caching and tp > 1:
+            raise ValueError("enable_prefix_caching is single-GPU only (tensor_parallel_size must be 1)")
+        if enable_prefix_caching and isinstance(model, ChatTSForCausalLM) and not model.enable_prefix_caching:
+            raise ValueError("enable_prefix_caching=True with a model built without it: construct it with enable_prefix_caching=True")
+        self._tp_procs, self._tp_driver = [], False
         tp_kw = {}
         if tp > 1:
             import torch.distributed as dist
@@ -198,12 +205,14 @@ class LLM:
             self.model = model
         elif isinstance(model, str):
             self.model = ChatTSForCausalLM.from_pretrained(model, torch_dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs,
-                                                           quantization=quantization, **tp_kw)
+                                                           quantization=quantization, enable_prefix_caching=enable_prefix_caching, **tp_kw)
         else:
             cfg = config or ChatTSConfig.chatts_14b()
-            self.model = (ChatTSForCausalLM(cfg, state_dict, dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs, **tp_kw)
+            pc = dict(enable_prefix_caching=True) if enable_prefix_caching else {}
+            self.model = (ChatTSForCausalLM(cfg, state_dict, dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs, **tp_kw, **pc)
                           if state_dict is not None else
-                          ChatTSForCausalLM.from_synthetic(cfg, seed=seed, dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs, **tp_kw))
+                          ChatTSForCausalLM.from_synthetic(cfg, seed=seed, dtype=dt, max_seq_len=max_model_len, max_batch=max_num_seqs, **tp_kw,
+                                                           **pc))
         if quantization == "fp8" and self.model.fp8 is None:
             self.model.quantize_fp8()
         cfg = self.model.config
@@ -238,7 +247,8 @@ class LLM:
             # n completions per request = n copies of the request in the batch, each row with its own draw
             # (llm_utils.py:127-130 reads outputs[i].outputs[j].text for j < n)
             flat = self._generate([r for r in inputs for _ in range(n)], sp)
-            return [RequestOutput(inputs[i]["prompt"], [flat[i * n + j].outputs[0] for j in range(n)]) for i in range(len(inputs))]
+            return [RequestOutput(inputs[i]["prompt"], [flat[i * n + j].outputs[0] for j in range(n)], flat[i * n].num_cached_tokens)
+                    for i in range(len(inputs))]
         return self._generate(inputs, sp, streamer)
 
     def _generate(self, inputs, sp, streamer=None):
@@ -273,7 +283,9 @@ class LLM:
                 # a row ends at ITS first stop id (the batch-wide tail after it is the pad fill of generate())
                 toks, fin = cut_at_stop(ids[b, S:].tolist(), stop_ids, sp.ignore_eos)
                 text, hit = cut_at_stop_string(decode_text(self.tokenizer, toks), stops)
-                outs.append(RequestOutput(req["prompt"], [CompletionOutput(text, toks, "stop" if hit else fin)]))
+                hits = getattr(self.model, "last_cached_positions", None)
+                outs.append(RequestOutput(req["prompt"], [CompletionOutput(text, toks, "stop" if hit else fin)],
+                                          int(hits[b]) if hits is not None else 0))
         return outs
 
 
@@ -296,6 +308,7 @@ class AsyncEngineArgs:
     trust_remote_code: bool = True
     dtype: str = "bfloat16"
     max_num_seqs: int = 1
+    enable_prefix_caching: bool = False
 
 
 class _AsyncStreamer:
@@ -319,7 +332,8 @@ class AsyncLLMEngine:
     def from_engine_args(cls, args, llm=None):
         if llm is None:
             llm = LLM(model=args.model, tensor_parallel_size=args.tensor_parallel_size, dtype=args.dtype, max_model_len=args.max_model_len,
-                      max_num_seqs=args.max_num_seqs, limit_mm_per_prompt=args.limit_mm_per_prompt, trust_remote_code=args.trust_remote_code)
+                      max_num_seqs=args.max_num_seqs, limit_mm_per_prompt=args.limit_mm_per_prompt, trust_remote_code=args.trust_remote_code,
+                      enable_prefix_caching=args.enable_prefix_caching)
         return cls(llm)
 
     async def generate(self, prompt, sampling_params=None, request_id=None):

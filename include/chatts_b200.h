@@ -166,6 +166,20 @@ int cts_attn_prefill(cts_ctx* ctx, const void* q, const void* k, const void* v, 
                      int max_seqlen, long long total_tokens, int nh, int nkv, int head_dim, float scale, void* out,
                      int dtype, void* stream);
 
+/* prefill against the PAGED cache: causal GQA for each sequence's new query rows over all its keys in the cache -- a cached prompt
+ * prefix plus the new rows, which cts_qkv_rope_cache has already written there (the prefill vLLM runs under enable_prefix_caching,
+ * which the reference switches off for time series, chatts/utils/llm_utils.py:154).
+ *   q [total_q, nh, d] packed by cu_q int32[batch+1]; kv_lens int32[batch]: keys of each sequence, the new rows included, so query row
+ *   i of sequence b sits at position kv_lens[b] - q_len_b + i and sees keys j <= that position; k_cache/v_cache
+ *   [num_pages, nkv, page_size, d], page_table int32[batch, max_pages]; out [total_q, nh*d].  page_size 16, 32 or 64; nh/nkv <= 8.
+ *   Key tiles start at position 0 for every row, so with kv_lens == q lens the output is cts_attn_prefill's bit for bit, and a row
+ *   gets the same bits in a suffix call as in a full prefill over the same cache contents.  Cache rows at or past kv_lens[b] are
+ *   never read into the result (their V rows are zeroed before the P V product).
+ */
+int cts_attn_prefill_paged(cts_ctx* ctx, const void* q, const int* cu_q, const int* kv_lens, const void* k_cache, const void* v_cache,
+                           int num_pages, const int* page_table, int max_pages, int batch, int max_q, long long total_q, int nh, int nkv,
+                           int head_dim, int page_size, float scale, void* out, int dtype, void* stream);
+
 /* decode: one query token per sequence against the paged cache (flash-decoding split over KV tiles of 64 tokens;
  * pages are staged by TMA with the 128-byte swizzle, QK^T and PV run on mma.sync, the last split to finish merges).
  *   q [batch, nh, d]; k_cache/v_cache [num_pages, nkv, page_size, d]; page_table int32[batch, max_pages];

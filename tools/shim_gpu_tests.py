@@ -124,6 +124,14 @@ SELECT = {
     # it does not own
     "test_gpu_zz_g_decode_parity.py": "tiny-default-b1-p16 or tiny-default-b8-p32-bf16 or tiny-default-b8-p32-fp16 or tiny-native-b8-p16-bf16 "
                                       "or (not_own and default and nan)",
+    # the paged prefill attention: short batches at one page size per GQA ratio, the bitwise cases at their small shapes
+    "test_gpu_attn_prefill_paged.py": "(matches_fp32 and short and ((16-4-2 and 16-) or (128-10-2 and 32-) or (64-16-2 and 64-))) "
+                                      "or (no_prefix and (1-64-65-300 or 5-64-129)) or (suffix and (200-64 or 130-1 or 64-63) and 10-2) "
+                                      "or foreign or argument_errors",
+    # prefix caching on the tiny model: cold = uncached bit for bit, a warm call against the oracle, a hit boundary inside a series,
+    # other series under the same ids, and the engine's shared-prefix admissions
+    "test_gpu_zz_h_prefix_cache.py": "(cold_call and tiny) or (warm_call and tiny-16-insert) or boundary_inside or (same_ids and tiny) "
+                                     "or (continuous_engine and bf16)",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
