@@ -32,7 +32,9 @@ SYMBOLS = [
     "cts_peer_ll_region_bytes", "cts_peer_allreduce_ll", "cts_trace_enable", "cts_ts_encode_fused_ok", "cts_ts_encode_fused",
     "cts_rep_penalty_mark", "cts_rep_penalty_apply", "cts_gemm_w4", "cts_gemm_w4_suggest_split", "cts_gemm_w4_mma", "cts_gemm_w4_mma_suggest_split",
     "cts_gemm_fp8", "cts_gemm_fp8_suggest_split", "cts_fp8_dequant", "cts_attn_prefill_paged",
+    "cts_logprobs_workspace_floats", "cts_logprobs",
 ]
+LOGPROBS_MAX_K = 20
 FUSED_RESIDUAL, FUSED_SWIGLU, FUSED_QKV_ROPE = 0, 1, 2
 PACK_DESC_LONGS = 12
 
@@ -196,6 +198,10 @@ def load_library():
         getattr(lib, name).restype = i
     lib.cts_sample_advance.argtypes = [vp, vp, ll, i, f, i, f, C.c_ulonglong, vp, i, vp, vp, vp, vp, vp, vp, i, i, i, vp]
     lib.cts_sample_advance.restype = i
+    lib.cts_logprobs_workspace_floats.argtypes = [i, ll, i]
+    lib.cts_logprobs_workspace_floats.restype = ll
+    lib.cts_logprobs.argtypes = [vp, vp, ll, ll, i, vp, i, vp, i, vp, vp, vp, vp, i, vp, vp, i, vp]
+    lib.cts_logprobs.restype = i
     # ---- A9: LoRA fine-tune step
     lib.cts_attn_prefill_lse.argtypes = [vp, vp, vp, vp, vp, i, i, ll, i, i, i, f, vp, vp, i, vp]
     lib.cts_attn_bwd.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i, i, ll, i, i, i, f, vp, vp, vp, vp, i, vp]
@@ -580,6 +586,21 @@ class Context:
                                               _p(positions), _p(seq_lens), _p(slot_map), _p(page_table),
                                               page_table.shape[1] if page_table is not None else 0, page_size,
                                               dtype_code(logits.dtype), _stream()))
+
+    def logprobs_workspace_floats(self, rows, vocab, k):
+        return int(self.lib.cts_logprobs_workspace_floats(int(rows), int(vocab), int(k)))
+
+    def logprobs(self, logits, rows, chosen, k, out_logprob, out_rank, out_topk_ids, out_topk_logprobs, workspace, counters,
+                 step_ptr=None, vocab=None):
+        """Log probabilities of rows x logits[:, :vocab] (cts_logprobs): the chosen id's logprob and rank and the k largest entries.
+        chosen int32 [rows, >= 1] and the outputs [rows, out_ld(, k)] are read / written at column step_ptr[0] - 1 (column 0 without
+        step_ptr); workspace float32 of logprobs_workspace_floats(rows, vocab, k), counters int32 [rows] zero-filled once."""
+        vocab = logits.shape[-1] if vocab is None else vocab
+        out_ld = out_logprob.stride(0) if out_logprob is not None else out_topk_ids.shape[1]
+        self._chk(self.lib.cts_logprobs(self.h, _p(logits), int(vocab), logits.stride(0), int(rows), _p(chosen),
+                                        chosen.stride(0) if chosen is not None else 0, _p(step_ptr), int(k), _p(out_logprob), _p(out_rank),
+                                        _p(out_topk_ids), _p(out_topk_logprobs), out_ld, _p(workspace), _p(counters),
+                                        dtype_code(logits.dtype), _stream()))
 
     def rep_penalty_mark(self, tokens, rows, seen, vocab):
         """Set the bits of (row, token) pairs in seen [B, words]; rows None: pair i belongs to row i."""

@@ -227,6 +227,221 @@ extern "C" int cts_sample_advance(cts_ctx* ctx, const void* logits, long long vo
 }
 
 // ------------------------------------------------------------------------------------------------
+// Log probabilities (vLLM's raw logprobs): per row, log_softmax of the 16-bit logits at the chosen id, the chosen id's rank, and the
+// k largest entries.  A row is cut into slices of kLpSlice logits, one CTA each; every CTA reduces its slice to (max, sum of exp,
+// count above the chosen logit, its k best (value, id) keys) in the workspace, and the last CTA of the row to arrive merges the
+// slices in slice order (so the result does not depend on arrival order) and resets the row's arrival counter.
+// ------------------------------------------------------------------------------------------------
+namespace {
+constexpr int kLpThreads = 256;
+constexpr int kLpPer = 8;                            // logits per thread: one 16-byte load
+constexpr int kLpSlice = kLpThreads * kLpPer;        // logits per CTA
+constexpr int kLpMaxK = 20;
+
+// a top-k key: the value's ordered bits above the complemented id, so the larger key is the larger value and, among equal values,
+// the smaller id; -0 is folded onto +0 (equal values tie).  0 is never a key (the smallest, -inf, has high word 0x007fffff).
+__device__ __forceinline__ unsigned long long lp_key(float x, int id) {
+  unsigned u = __float_as_uint(x);
+  if ((u << 1) == 0u) u = 0u;
+  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return ((unsigned long long)u << 32) | (unsigned)~(unsigned)id;
+}
+__device__ __forceinline__ float lp_key_value(unsigned long long key) {
+  const unsigned u = (unsigned)(key >> 32);
+  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+__device__ __forceinline__ int lp_key_id(unsigned long long key) { return (int)~(unsigned)key; }
+
+// (max, sum of exp(x - max)) of two parts; NaN never enters, -inf contributes nothing
+__device__ __forceinline__ void lp_merge(float& m, float& s, float m2, float s2) {
+  const float mm = fmaxf(m, m2);
+  if (mm == -INFINITY) { m = mm; s = 0.f; return; }
+  s = (m == mm ? s : s * expf(m - mm)) + (m2 == mm ? s2 : s2 * expf(m2 - mm));
+  m = mm;
+}
+
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
+    v = w > v ? w : v;
+  }
+  return v;
+}
+__device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v, unsigned long long* red) {
+  v = warp_max_u64(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  v = threadIdx.x < kLpThreads / 32 ? red[threadIdx.x] : 0ull;
+  if (threadIdx.x < 32) v = warp_max_u64(v);
+  if (threadIdx.x == 0) red[0] = v;
+  __syncthreads();
+  return red[0];
+}
+// block-wide (max, sum, count), combined in a fixed tree
+__device__ __forceinline__ void block_lp_stats(float& m, float& s, int& c, float* fred, int* cred) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    c += __shfl_xor_sync(0xffffffffu, c, o);
+    lp_merge(m, s, m2, s2);
+  }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) { fred[threadIdx.x >> 5] = m; fred[32 + (threadIdx.x >> 5)] = s; cred[threadIdx.x >> 5] = c; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kLpThreads / 32; ++w) { lp_merge(m, s, fred[w], fred[32 + w]); c += cred[w]; }
+    fred[0] = m; fred[32] = s; cred[0] = c;
+  }
+  __syncthreads();
+  m = fred[0]; s = fred[32]; c = cred[0];
+}
+
+// one slice record in the workspace: {max, sum} {count, -} then k keys (8-byte words)
+template <typename T>
+__global__ void __launch_bounds__(kLpThreads)
+logprobs_kernel(const T* __restrict__ logits, long long vocab, long long ld, const int* __restrict__ chosen, int chosen_ld,
+                const int* __restrict__ step_ptr, int k, float* __restrict__ out_logprob, int* __restrict__ out_rank,
+                int* __restrict__ out_topk_ids, float* __restrict__ out_topk_logprobs, int out_ld, int* __restrict__ counters,
+                unsigned long long* __restrict__ records) {
+  pdl_trigger();
+  pdl_wait();
+  __shared__ float fred[64];
+  __shared__ int cred[32];
+  __shared__ unsigned long long kred[32];
+  __shared__ int last_s;
+  const int slice = blockIdx.x, nslice = gridDim.x, r = blockIdx.y;
+  const T* row = logits + (long long)r * ld;
+  const int col = step_ptr ? step_ptr[0] - 1 : 0;
+  const int cid = chosen ? chosen[(long long)r * chosen_ld + col] : -1;
+  const float xc = (cid >= 0 && cid < vocab) ? DT<T>::to_f(row[cid]) : NAN;
+
+  // ---- this CTA's slice: 8 logits per thread
+  const long long i0 = (long long)slice * kLpSlice + (long long)threadIdx.x * kLpPer;
+  float x[kLpPer];
+  if (i0 + kLpPer <= vocab && (ld & 7) == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
+    const uint4 u = *reinterpret_cast<const uint4*>(row + i0);
+    const T* p = reinterpret_cast<const T*>(&u);
+#pragma unroll
+    for (int j = 0; j < kLpPer; ++j) x[j] = DT<T>::to_f(p[j]);
+  } else {
+#pragma unroll
+    for (int j = 0; j < kLpPer; ++j) x[j] = i0 + j < vocab ? DT<T>::to_f(row[i0 + j]) : NAN;
+  }
+  float m = -INFINITY, s = 0.f;
+  int c = 0;
+#pragma unroll
+  for (int j = 0; j < kLpPer; ++j) {
+    const float v = x[j];
+    if (v != v) continue;                                                    // NaN: no mass, no rank, not a candidate
+    c += v > xc;
+    if (v > m) { s = s * expf(m - v) + 1.f; m = v; }
+    else if (v != -INFINITY) s += expf(v - m);
+  }
+  block_lp_stats(m, s, c, fred, cred);
+  unsigned long long* rec = records + ((long long)r * nslice + slice) * (2 + k);
+  if (threadIdx.x == 0) {
+    rec[0] = ((unsigned long long)__float_as_uint(s) << 32) | __float_as_uint(m);
+    rec[1] = (unsigned)c;
+  }
+  // k best of the slice: k rounds of a block max over each thread's best key below the previous winner
+  auto best_below = [&](unsigned long long lim) {
+    unsigned long long b = 0ull;
+#pragma unroll
+    for (int j = 0; j < kLpPer; ++j) {
+      if (x[j] == x[j]) {
+        const unsigned long long kk = lp_key(x[j], (int)(i0 + j));
+        if (kk < lim && kk > b) b = kk;
+      }
+    }
+    return b;
+  };
+  unsigned long long mine = k > 0 ? best_below(~0ull) : 0ull;
+  for (int j = 0; j < k; ++j) {
+    const unsigned long long w = block_max_u64(mine, kred);
+    if (threadIdx.x == 0) rec[2 + j] = w;
+    if (w != 0ull && mine == w) mine = best_below(w);                        // keys are unique: one thread moves on
+  }
+
+  // ---- the last CTA of the row merges the slices
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last_s = atomicAdd(&counters[r], 1) == nslice - 1;
+  }
+  __syncthreads();
+  if (!last_s) return;
+  __threadfence();
+  const unsigned long long* recs = records + (long long)r * nslice * (2 + k);
+  m = -INFINITY; s = 0.f; c = 0;
+  for (int q = threadIdx.x; q < nslice; q += kLpThreads) {
+    const unsigned long long a = __ldcg(recs + (long long)q * (2 + k));
+    lp_merge(m, s, __uint_as_float((unsigned)a), __uint_as_float((unsigned)(a >> 32)));
+    c += (int)(unsigned)__ldcg(recs + (long long)q * (2 + k) + 1);
+  }
+  block_lp_stats(m, s, c, fred, cred);
+  const float log_s = logf(s);
+  const long long o = (long long)r * out_ld + col;
+  if (threadIdx.x == 0) {
+    if (out_logprob) out_logprob[o] = (xc - m) - log_s;
+    if (out_rank) out_rank[o] = xc == xc ? 1 + c : 0;
+    counters[r] = 0;                                                         // ready for the next launch (graph replays included)
+  }
+  const long long ncand = (long long)nslice * k;
+  auto cand_below = [&](unsigned long long lim) {
+    unsigned long long b = 0ull;
+    for (long long q = threadIdx.x; q < ncand; q += kLpThreads) {
+      const unsigned long long kk = __ldcg(recs + (q / k) * (2 + k) + 2 + q % k);
+      if (kk < lim && kk > b) b = kk;
+    }
+    return b;
+  };
+  mine = k > 0 ? cand_below(~0ull) : 0ull;
+  for (int j = 0; j < k; ++j) {
+    const unsigned long long w = block_max_u64(mine, kred);
+    if (threadIdx.x == 0) {
+      out_topk_ids[o * k + j] = w ? lp_key_id(w) : -1;
+      out_topk_logprobs[o * k + j] = w ? (lp_key_value(w) - m) - log_s : NAN;
+    }
+    if (w != 0ull && mine == w) mine = cand_below(w);
+  }
+}
+}  // namespace
+
+extern "C" long long cts_logprobs_workspace_floats(int rows, long long vocab, int k) {
+  if (rows <= 0 || vocab <= 0 || k < 0) return 0;
+  const long long nslice = (vocab + kLpSlice - 1) / kLpSlice;
+  return (long long)rows * nslice * (2 + k) * 2;
+}
+
+extern "C" int cts_logprobs(cts_ctx* ctx, const void* logits, long long vocab, long long ld, int rows, const int* chosen, int chosen_ld,
+                            const int* step_ptr, int k, float* out_logprob, int* out_rank, int* out_topk_ids, float* out_topk_logprobs,
+                            int out_ld, float* workspace, int* counters, int dtype, void* stream) {
+  if (!ctx) return CTS_ERR_BAD_ARG;
+  CTS_CHECK_ARG(ctx, vocab > 0 && vocab <= (1LL << 24) && ld >= vocab && rows >= 0 && rows <= 65535, "vocab (<= 2^24) / ld (>= vocab) / rows (<= 65535)");
+  CTS_CHECK_ARG(ctx, k >= 0 && k <= kLpMaxK, "k must be in [0, 20]");
+  CTS_CHECK_ARG(ctx, dtype == CTS_BF16 || dtype == CTS_F16, "dtype");
+  if (rows == 0) return CTS_OK;
+  CTS_CHECK_ARG(ctx, logits != nullptr && workspace != nullptr && counters != nullptr, "null logits / workspace / counters");
+  CTS_CHECK_ARG(ctx, (reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "workspace must be 8-byte aligned");
+  CTS_CHECK_ARG(ctx, (out_logprob == nullptr && out_rank == nullptr) || (chosen != nullptr && chosen_ld >= 1), "chosen ids for the chosen logprob / rank");
+  CTS_CHECK_ARG(ctx, k == 0 || (out_topk_ids != nullptr && out_topk_logprobs != nullptr), "null top-k outputs");
+  CTS_CHECK_ARG(ctx, out_ld >= 1, "out_ld");
+  const long long nslice = (vocab + kLpSlice - 1) / kLpSlice;
+  auto* records = reinterpret_cast<unsigned long long*>(workspace);
+  const dim3 grid((unsigned)nslice, (unsigned)rows);
+  if (dtype == CTS_BF16)
+    CTS_CUDA(ctx, launch_pdl(logprobs_kernel<__nv_bfloat16>, grid, dim3(kLpThreads), 0, (cudaStream_t)stream, 1, (const __nv_bfloat16*)logits,
+                             vocab, ld, chosen, chosen_ld, step_ptr, k, out_logprob, out_rank, out_topk_ids, out_topk_logprobs, out_ld, counters,
+                             records));
+  else
+    CTS_CUDA(ctx, launch_pdl(logprobs_kernel<__half>, grid, dim3(kLpThreads), 0, (cudaStream_t)stream, 1, (const __half*)logits, vocab, ld,
+                             chosen, chosen_ld, step_ptr, k, out_logprob, out_rank, out_topk_ids, out_topk_logprobs, out_ld, counters, records));
+  return CTS_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Repetition penalty (transformers RepetitionPenaltyLogitsProcessor; the checkpoint's generation_config.json may set it): for every
 // token id that already occurs in the row's sequence -- prompt and generated part -- logit = logit / penalty if logit > 0 else
 // logit * penalty, applied ONCE however often the token occurred.  The occurrence set is a bit mask [batch, ceil(vocab / 32)]:

@@ -21,6 +21,9 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
+from . import logprobs as lpmod
+from ._cabi import LOGPROBS_MAX_K
+
 
 @dataclass
 class Request:
@@ -36,6 +39,8 @@ class Request:
     done: bool = False
     error: Exception = None            # set when the request could not be admitted (over-long, or larger than the whole KV pool)
     cached_positions: int = 0          # prompt positions whose KV came from the prefix cache (model built with enable_prefix_caching)
+    logprobs: int = None               # top-k of the logprobs asked for (None: none)
+    token_logprobs: list = field(default_factory=list)   # per token: (logprob, rank, top-k ids, top-k logprobs), as in generate()
 
 
 class ContinuousEngine:
@@ -60,15 +65,18 @@ class ContinuousEngine:
         self._reset_free(list(range(self.B)))
         self.rounds = 0
         self.occupancy = []                                # active slots per round (observability / tests)
+        self._lpb = None                                   # logprob outputs of a round, made when a request first asks
 
     # ------------------------------------------------------------------------------------------ public
-    def add_request(self, input_ids, series=None, max_new_tokens=16, eos_token_id=None, ignore_eos=False):
+    def add_request(self, input_ids, series=None, max_new_tokens=16, eos_token_id=None, ignore_eos=False, logprobs=None):
+        """logprobs = k (0..20): every token's logprob and rank and the k most likely tokens, in Request.token_logprobs."""
+        k = lpmod.check_k(logprobs, "logprobs")
         cfg = self.m.config
         eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
         eos = set(eos) if isinstance(eos, (list, tuple, set)) else {int(eos)}
         ids = torch.as_tensor(input_ids, dtype=torch.long).reshape(-1)
         ts = series if series is not None else torch.zeros(0, 0, 1)
-        r = Request(self._next, ids, ts, int(max_new_tokens), eos, ignore_eos)
+        r = Request(self._next, ids, ts, int(max_new_tokens), eos, ignore_eos, logprobs=k)
         self._next += 1
         self.waiting.append(r)
         return r.rid
@@ -170,7 +178,13 @@ class ContinuousEngine:
             t_slot = torch.zeros(g, dtype=torch.int32, device=dev)
             t_pt = torch.from_numpy(pts).to(dev)
             m.ctx.greedy_advance(logits, g, t_out, t_step, t_cur, t_pos, t_seq, t_slot, t_pt, m.page_size)
+            ks = [r.logprobs for r in group if r.logprobs is not None]
+            if ks:                                         # the first token's logprobs, from the prefill logits
+                lpb = lpmod.LogprobBuffers(m.ctx, g, 1, max(ks), m.config.vocab_size, dev)
+                lpb.launch(logits, g, t_out, step_ptr=t_step)
             first = t_out[:, 0].cpu().tolist()             # host read: the request's first token (and EOS check)
+            if ks:
+                first_lp = lpb.host(1)
             slots = torch.tensor(free[:g], device=dev)
             st = self.st
             st.cur_ids[slots], st.positions[slots], st.seq_lens[slots], st.slot_map[slots] = t_cur, t_pos, t_seq, t_slot
@@ -181,6 +195,8 @@ class ContinuousEngine:
                 r.slot = free[i]
                 r.cached_positions = int(cached[i]) if cached is not None else 0
                 r.tokens.append(int(first[i]))
+                if r.logprobs is not None:
+                    r.token_logprobs.append(self._entry(first_lp, i, 0, r.logprobs))
                 self.active[r.slot] = r
                 self._check_done(r)
             free = free[g:]
@@ -210,9 +226,15 @@ class ContinuousEngine:
         if free:
             self._reset_free(free)
         st.step_ptr.zero_()
+        ks = [r.logprobs for r in self.active.values() if r.logprobs is not None]
+        if ks and self._lpb is None:
+            self._lpb = lpmod.LogprobBuffers(m.ctx, self.B, self.k, LOGPROBS_MAX_K, m.config.vocab_size, m.device)
         for _ in range(self.k):
             m._decode_step(st, sample=True)
+            if ks:                                         # all slots at the largest k asked; columns from step_ptr
+                self._lpb.launch(st.full_logits, self.B, st.out_tokens, k=max(ks), step_ptr=st.step_ptr)
         toks = st.out_tokens[:, : self.k].cpu().numpy()    # the round's one device->host read
+        lps = self._lpb.host(self.k, max(ks)) if ks else None
         self.occupancy.append(len(self.active))
         out = []
         for slot, r in list(self.active.items()):
@@ -220,11 +242,18 @@ class ContinuousEngine:
                 if r.done:
                     break
                 r.tokens.append(int(toks[slot, j]))
+                if r.logprobs is not None:
+                    r.token_logprobs.append(self._entry(lps, slot, j, r.logprobs))
                 self._check_done(r)
             if r.done:
                 self._retire(r)
                 out.append(r)
         return out
+
+    @staticmethod
+    def _entry(host, row, col, k):
+        lp, rank, ids, vals = host
+        return float(lp[row, col]), int(rank[row, col]), ids[row, col, :k].tolist(), vals[row, col, :k].tolist()
 
     def _check_done(self, r):
         if len(r.tokens) >= r.max_new_tokens or (not r.ignore_eos and r.tokens[-1] in r.eos):

@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _cabi, layout, prefix_cache
+from . import logprobs as lpmod
 from .trace import span
 from ._cabi import EPI_NONE, EPI_PARTIAL_F32, EPI_RESIDUAL, EPI_SWIGLU_IL
 from .config import ChatTSConfig
@@ -727,13 +728,14 @@ class ChatTSForCausalLM:
         import os as _os
         return _os.environ.get("CTS_TS_MERGE_MODE") or getattr(self.config, "ts_merge_mode", "insert")
 
-    def _prefill(self, lay, counts, timeseries, page_tables, all_logits=False, cached=None):
+    def _prefill(self, lay, counts, timeseries, page_tables, all_logits=False, cached=None, prompt_lp=None):
         """Runs the prompt through the TS encoder + decoder, fills the paged KV cache, returns logits
         ([B,V] last position, or [T,V] for every merged position when all_logits).  ``cached`` (prefix caching, from _alloc_prompt):
-        per sequence, the number of leading positions whose KV the pages of ``page_tables`` already hold; only the rest is computed."""
+        per sequence, the number of leading positions whose KV the pages of ``page_tables`` already hold; only the rest is computed.
+        ``prompt_lp`` = k: also the prompt logprobs -- returns (logits, (targets, rows, cols, LogprobBuffers of the targets))."""
         if cached is not None and int(np.max(cached, initial=0)) > 0:
-            if all_logits:
-                raise ValueError("all_logits needs every position computed: no prefix-cache hits")
+            if all_logits or prompt_lp is not None:
+                raise ValueError("all_logits / prompt logprobs need every position computed: no prefix-cache hits")
             return self._prefill_suffix(lay, counts, timeseries, page_tables, np.asarray(cached, dtype=np.int64))
         c, dev, dt = self.ctx, self.device, self.dtype
         T, B = lay.total, lay.cu_seqlens.shape[0] - 1
@@ -760,6 +762,7 @@ class ChatTSForCausalLM:
             c.attn_prefill(st.q, st.k_lin, st.v_lin, cu_d, B, max_len, self.nh, self.nkv, self.d, scale, st.ao)
 
         self._layers(st, T, attend)
+        plp = None if prompt_lp is None else self._prompt_logprobs(lay, st.xn, prompt_lp)
         if all_logits:
             hn = st.xn
         else:
@@ -767,7 +770,31 @@ class ChatTSForCausalLM:
             hn = st.xn.index_select(0, last).contiguous()        # row gather of B rows (plumbing)
         logits = torch.empty(hn.shape[0], self.V, device=dev, dtype=dt)
         c.gemm(hn, self.lm_head, logits, epilogue=EPI_NONE)
+        if plp is not None:
+            return logits, plp
         return self._gather_vocab(logits)
+
+    PROMPT_LP_CHUNK = 1024
+
+    def _prompt_logprobs(self, lay, xn, k):
+        """Prompt logprobs from the final-norm rows xn [T, H] of a prefill: only the positions that predict a prompt token go through
+        the lm_head (patch rows that predict a patch row are skipped), in chunks of at most PROMPT_LP_CHUNK rows into one reused logits
+        buffer, then cts_logprobs with the next ids as the chosen ids.  -> (targets, rows, cols, LogprobBuffers [N, 1])."""
+        dev = self.device
+        pred, tgt, rows, cols = lpmod.prompt_targets(lay)
+        N = int(pred.shape[0])
+        chunk = min(self.PROMPT_LP_CHUNK, max(N, 1))
+        buf = lpmod.LogprobBuffers(self.ctx, max(N, 1), 1, k, self.V, dev, launch_rows=chunk)
+        if N:
+            idx = torch.from_numpy(np.stack([pred.astype(np.int32), tgt])).to(dev, non_blocking=True)
+            pred_d, tgt_d = idx[0].long(), idx[1].view(N, 1)
+            logits = torch.empty(chunk, self.V, device=dev, dtype=self.dtype)
+            for r0 in range(0, N, chunk):
+                n = min(chunk, N - r0)
+                hn = xn.index_select(0, pred_d[r0:r0 + n])                   # row gather of the predicting positions (plumbing)
+                self.ctx.gemm(hn, self.lm_head, logits, epilogue=EPI_NONE, t=n)
+                buf.launch(logits, n, tgt_d[r0:r0 + n], row0=r0)
+        return tgt, rows, cols, buf
 
     def _prefill_suffix(self, lay, counts, timeseries, page_tables, cached):
         """_prefill of the positions past each sequence's cached prefix: the embeddings, the series that have a patch row among them and
@@ -838,10 +865,11 @@ class ChatTSForCausalLM:
                     cached_pages=len(pool.page_of) if self.enable_prefix_caching else 0,
                     evictions=pool.evictions if self.enable_prefix_caching else 0)
 
-    def _alloc_prompt(self, lay, timeseries, extra):
+    def _alloc_prompt(self, lay, timeseries, extra, lookup=True):
         """Pages for the prompts of ``lay`` plus ``extra`` decode positions each: (page_tables, held, keys, cached).  With prefix
         caching on, the leading full pages an earlier prefill indexed are shared (cached = positions per sequence they hold) and keys
-        are what _prefix_register indexes once the prefill is enqueued; off, keys and cached are None."""
+        are what _prefix_register indexes once the prefill is enqueued; off, keys and cached are None.  lookup=False: no page is
+        shared (every position is computed), the keys are still returned for indexing."""
         if not self.enable_prefix_caching:
             return self._alloc_pages(lay.lens, extra) + (None, None)
         cnt = self._host_counts[1].numpy() if lay.row_map.shape[0] > 0 else np.zeros(0, dtype=np.int64)
@@ -849,7 +877,7 @@ class ChatTSForCausalLM:
         keys = prefix_cache.page_keys(lay, prefix_cache.series_digests(timeseries) if cnt.shape[0] else [], cnt, seed, self.page_size)
         needs = self._page_needs(lay.lens, extra)
         pool, ps = self.pool, self.page_size
-        hits = [pool.lookup(keys[b][: (int(n) - 1) // ps]) for b, n in enumerate(lay.lens)]
+        hits = [pool.lookup(keys[b][: (int(n) - 1) // ps]) if lookup else [] for b, n in enumerate(lay.lens)]
         hit_set = {p for h in hits for p in h}
         new = sum(n - len(h) for n, h in zip(needs, hits))
         # all-or-nothing: hits + free + evictable (minus the evictable pages this batch hits) against the need, before any reference
@@ -1068,10 +1096,22 @@ class ChatTSForCausalLM:
     @torch.no_grad()
     def generate(self, input_ids=None, attention_mask=None, timeseries=None, max_new_tokens=None, max_length=None,
                  do_sample=None, temperature=None, top_p=None, top_k=None, streamer=None, eos_token_id=None, pad_token_id=None,
-                 synced_gpus=False, sync_every=16, ignore_eos=False, seed=None, repetition_penalty=None, **_):
+                 synced_gpus=False, sync_every=16, ignore_eos=False, seed=None, repetition_penalty=None, logprobs=None,
+                 prompt_logprobs=None, **_):
         """model.generate(**processor_out, max_new_tokens=...) -> LongTensor [B, S + new] whose first S columns are
-        the ORIGINAL (un-expanded) input ids (README.md:102-103)."""
+        the ORIGINAL (un-expanded) input ids (README.md:102-103).
+
+        logprobs = k (0..20): every generated token's log probability and rank, and the k most likely tokens with theirs;
+        prompt_logprobs = k: the same for every prompt token after the first.  They go to ``self.last_logprobs``
+        (chatts_b200.logprobs.GenerationLogprobs; None when neither was asked).  They describe the distribution the token was picked
+        from: log_softmax in fp32 of the logits, after the repetition penalty when one is set and before temperature, top-k and top-p
+        (vLLM's raw logprobs whenever repetition_penalty == 1).  A call with prompt_logprobs computes every prompt position (no
+        prefix-cache hits; its pages are still indexed).  Single GPU only."""
         cfg, dev = self.config, self.device
+        lpk, plk = lpmod.check_k(logprobs, "logprobs"), lpmod.check_k(prompt_logprobs, "prompt_logprobs")
+        if (lpk is not None or plk is not None) and self.tp_size > 1:
+            raise ValueError("logprobs / prompt_logprobs are single-GPU only (tensor_parallel_size must be 1)")
+        self.last_logprobs = None
         gd = getattr(self, "generation_defaults", None)
         if gd:                                          # checkpoint defaults apply only where the caller said nothing
             if do_sample is None and gd.get("do_sample"):
@@ -1108,10 +1148,13 @@ class ChatTSForCausalLM:
                 box = [seed]
                 torch.distributed.broadcast_object_list(box, src=0, group=self.comm)
                 seed = int(box[0])
-        page_tables, held, keys, cached = self._alloc_prompt(lay, timeseries, max_new_tokens)
+        page_tables, held, keys, cached = self._alloc_prompt(lay, timeseries, max_new_tokens, lookup=plk is None)
         try:
             with span("cts.prefill"):
-                logits = self._prefill(lay, counts, timeseries, page_tables, cached=cached)
+                logits = self._prefill(lay, counts, timeseries, page_tables, cached=cached, prompt_lp=plk)
+            plp = None
+            if plk is not None:
+                logits, plp = logits
             self._prefix_register(keys, page_tables, lay.lens, cached)
             self.last_cached_positions = cached          # per row: prompt positions whose KV came from the prefix cache (None: caching off)
             st = self._decode_state(B, max_new_tokens)
@@ -1157,7 +1200,20 @@ class ChatTSForCausalLM:
                 if seen is not None:
                     self.ctx.rep_penalty_mark(st.cur_ids, None, seen, self.config.vocab_size)
 
+            # logprobs: one cts_logprobs launch after each advance, over the logits the token was picked from; the kernel advances
+            # (greedy, sample) leave step_ptr one past the column they wrote, the torch sampler does not move it.  Only called when
+            # asked: under tensor parallelism (refused above) the vocab-parallel greedy step leaves no full_logits.
+            lpb = None if lpk is None else lpmod.LogprobBuffers(self.ctx, B, max_new_tokens, lpk, self.config.vocab_size, dev)
+
+            def take_logprobs(lg, step):
+                if greedy or self.use_sample_kernel:
+                    lpb.launch(lg, B, st.out_tokens, step_ptr=st.step_ptr)
+                else:
+                    lpb.launch(lg, B, st.out_tokens, col=step)
+
             advance(logits, 0)
+            if lpb is not None:
+                take_logprobs(logits, 0)
             done = np.zeros(B, dtype=bool)
             out = np.full((B, max_new_tokens), pad, dtype=np.int64)
             emitted = 0
@@ -1185,6 +1241,8 @@ class ChatTSForCausalLM:
                         if seen is not None:
                             self.ctx.rep_penalty_apply(st.full_logits, B, seen, rep)
                         advance(st.full_logits, produced)
+                    if lpb is not None:
+                        take_logprobs(st.full_logits, produced)
                 produced += 1
             if streamer is not None:
                 streamer.end()
@@ -1193,6 +1251,14 @@ class ChatTSForCausalLM:
         is_eos = np.isin(out[:, :emitted], list(eos_set)) if not ignore_eos else np.zeros((B, emitted), dtype=bool)
         first = np.where(is_eos.any(axis=1), is_eos.argmax(axis=1) + 1, emitted)
         n_out = int(min(max(first.max(), 1), max_new_tokens))
+        if lpk is not None or plk is not None:
+            res = lpmod.GenerationLogprobs()
+            if lpb is not None:
+                res.logprobs, res.ranks, res.top_ids, res.top_logprobs = lpb.host(n_out)
+            if plp is not None:
+                tgt, rows, cols, pbuf = plp
+                res.prompt = lpmod.prompt_entries(ids_cpu, am_cpu, rows, cols, tgt, *(a[:, 0] for a in pbuf.host(1)))
+            self.last_logprobs = res
         return torch.cat([torch.as_tensor(ids_cpu, dtype=torch.long), torch.as_tensor(out[:, :n_out])], dim=1)
 
     def _sample_advance(self, st, logits, step, temperature, top_p, gen, top_k=None):

@@ -22,7 +22,8 @@ import uuid
 from concurrent.futures import Future
 from dataclasses import dataclass, field
 
-from .vllm_compat import IncrementalDecoder, eos_ids
+from .logprobs import check_k
+from .vllm_compat import IncrementalDecoder, decode_text, eos_ids
 
 MAX_TS_DEFAULT = 15          # scripts/start_vllm_server.sh:9  (--limit-mm-per-prompt timeseries=15)
 
@@ -147,7 +148,8 @@ class Engine:
         """Iteration-level batching (engine.ContinuousEngine): requests join the static decode slots between graph replays and
         leave them at EOS / max_tokens; streaming requests get their new tokens after every round."""
         from .engine import ContinuousEngine
-        from .vllm_compat import CompletionOutput, RequestOutput, cut_at_stop, cut_at_stop_string, decode_text
+        from .vllm_compat import (CompletionOutput, RequestOutput, cut_at_stop, cut_at_stop_string, decode_text, logprob_dict,
+                                  tokens_before_stop_string)
         llm = self.llm
         eng = ContinuousEngine(llm.model, steps_per_round=self.steps_per_round)
         jobs, sent = {}, {}
@@ -159,7 +161,7 @@ class Engine:
                 gd = getattr(llm.model, "generation_defaults", None) or {}
                 job.stop_ids = eos_ids(llm.model.config, p.get("stop_token_ids"), gd.get("eos_token_id"))
                 rid = eng.add_request(enc["input_ids"][0], enc["timeseries"], max_new_tokens=p.get("max_tokens", 16),
-                                      eos_token_id=job.stop_ids, ignore_eos=p.get("ignore_eos", False))
+                                      eos_token_id=job.stop_ids, ignore_eos=p.get("ignore_eos", False), logprobs=p.get("logprobs"))
                 jobs[rid], sent[rid] = job, 0
                 if job.stream_q is not None:
                     job.decoder = IncrementalDecoder(llm.tokenizer)
@@ -168,10 +170,16 @@ class Engine:
                 if job.stream_q is not None:
                     job.stream_q.put(None)
 
-        def finish(job, tokens):
-            toks, fin = cut_at_stop(tokens, job.stop_ids, job.params.get("ignore_eos", False))
-            text, hit = cut_at_stop_string(decode_text(llm.tokenizer, toks), job.params.get("stop") or [])
-            return CompletionOutput(text, toks, "stop" if hit else fin)
+        def finish(job, r):
+            toks, fin = cut_at_stop(r.tokens, job.stop_ids, job.params.get("ignore_eos", False))
+            stops = job.params.get("stop") or []
+            text, hit = cut_at_stop_string(decode_text(llm.tokenizer, toks), stops)
+            out = CompletionOutput(text, toks, "stop" if hit else fin)
+            if r.logprobs is not None:
+                keep = tokens_before_stop_string(llm.tokenizer, toks, stops) if hit else len(toks)
+                out.logprobs = [logprob_dict(toks[j], *r.token_logprobs[j], llm.tokenizer) for j in range(keep)]
+                out.cumulative_logprob = float(sum(r.token_logprobs[j][0] for j in range(keep)))
+            return out
 
         while not self.stop:
             if not eng.has_work():
@@ -219,7 +227,7 @@ class Engine:
                         job.stream_q.put(None)
                     continue
                 n = max(1, int(job.params.get("n", 1)))
-                out = finish(job, r.tokens)
+                out = finish(job, r)
                 job.future.set_result(RequestOutput(job.prompt, [out] * n))
                 if job.stream_q is not None:
                     tail = job.decoder.flush()
@@ -250,7 +258,9 @@ class _QueueStreamer:
             self.q.put(tail)
 
 
-def _sampling_from_body(body):
+def _sampling_from_body(body, chat=False):
+    """SamplingParams fields of an OpenAI request body.  Log probabilities: chat takes ``logprobs: true`` with ``top_logprobs`` 0..20,
+    completions ``logprobs: <int>`` 0..20; neither works with ``stream`` (ValueError, a 400 for the client)."""
     p = {"max_tokens": int(body.get("max_tokens") or body.get("max_completion_tokens") or 256),
          "temperature": float(body.get("temperature", 0.0) or 0.0), "top_p": float(body.get("top_p", 1.0) or 1.0),
          "top_k": int(body.get("top_k", 0) or 0), "n": int(body.get("n", 1) or 1)}
@@ -263,7 +273,46 @@ def _sampling_from_body(body):
         p["seed"] = int(body["seed"])
     if body.get("ignore_eos"):
         p["ignore_eos"] = True
+    if chat:
+        want = body.get("logprobs")
+        if want not in (None, False, True):
+            raise ValueError("logprobs must be a boolean in a chat completion request")
+        k = body.get("top_logprobs")
+        if k is not None and not want:
+            raise ValueError("top_logprobs needs logprobs: true")
+        k = (0 if k is None else k) if want else None
+    else:
+        k = body.get("logprobs")
+    if k is not None:
+        p["logprobs"] = check_k(k, "top_logprobs" if chat else "logprobs")
+        if body.get("stream"):
+            raise ValueError("logprobs are not available on streamed responses: send the request with stream=false")
     return p
+
+
+def _token_entry(tokenizer, tid, lp):
+    text = decode_text(tokenizer, [int(tid)])
+    return text, {"token": text, "logprob": lp.logprob, "bytes": list(text.encode("utf-8"))}
+
+
+def _response_logprobs(tokenizer, c, k, chat):
+    """The OpenAI ``logprobs`` object of one choice from CompletionOutput.logprobs (top-k: by logprob, then the smaller id)."""
+    content, tokens, token_lps, tops, offsets = [], [], [], [], []
+    for j, d in enumerate(c.logprobs or []):
+        tid = c.token_ids[j]
+        text, ent = _token_entry(tokenizer, tid, d[tid])
+        top = sorted(d.items(), key=lambda kv: (-kv[1].logprob, kv[0]))[:k]
+        if chat:
+            ent["top_logprobs"] = [_token_entry(tokenizer, i, v)[1] for i, v in top]
+            content.append(ent)
+        else:
+            offsets.append(len(decode_text(tokenizer, c.token_ids[:j])))
+            tokens.append(text)
+            token_lps.append(d[tid].logprob)
+            tops.append({_token_entry(tokenizer, i, v)[0]: v.logprob for i, v in top})
+    if chat:
+        return {"content": content}
+    return {"tokens": tokens, "token_logprobs": token_lps, "top_logprobs": tops, "text_offset": offsets}
 
 
 def create_app(llm, served_model_name="chatts", batch_window_ms=5.0, max_ts_per_prompt=MAX_TS_DEFAULT, scheduler="batch",
@@ -290,7 +339,10 @@ def create_app(llm, served_model_name="chatts", batch_window_ms=5.0, max_ts_per_
 
     async def run(prompt, series, body, chat):
         import asyncio
-        params = _sampling_from_body(body)
+        try:
+            params = _sampling_from_body(body, chat)
+        except (ValueError, TypeError) as e:
+            raise HTTPException(400, str(e))
         rid = ("chatcmpl-" if chat else "cmpl-") + uuid.uuid4().hex[:24]
         created = int(time.time())
         n_ph = prompt.count("<ts><ts/>")
@@ -326,6 +378,8 @@ def create_app(llm, served_model_name="chatts", batch_window_ms=5.0, max_ts_per_
             fin = c.finish_reason or ("length" if len(c.token_ids) >= params["max_tokens"] else "stop")
             choices.append({"index": i, "message": {"role": "assistant", "content": c.text}, "finish_reason": fin} if chat else
                            {"index": i, "text": c.text, "finish_reason": fin})
+            if "logprobs" in params:
+                choices[-1]["logprobs"] = _response_logprobs(llm.tokenizer, c, params["logprobs"], chat)
         return JSONResponse({"id": rid, "object": "chat.completion" if chat else "text_completion", "created": created,
                              "model": served_model_name, "choices": choices, "usage": usage(prompt, out.outputs)})
 

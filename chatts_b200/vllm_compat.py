@@ -9,6 +9,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
+from . import logprobs as lpmod
 from .config import ChatTSConfig
 from .model import ChatTSForCausalLM
 from .processor import ChatTSProcessor, SimpleTokenizer
@@ -30,6 +31,20 @@ class SamplingParams:
     ignore_eos: bool = False
     seed: int = None
     repetition_penalty: float = 1.0                   # vLLM SamplingParams.repetition_penalty (prompt + generated tokens)
+    logprobs: int = None                              # 0..20: logprob of every generated token plus its top-k (single GPU)
+    prompt_logprobs: int = None                       # 0..20: the same for every prompt token after the first (single GPU)
+
+    def __post_init__(self):
+        lpmod.check_k(self.logprobs, "logprobs")
+        lpmod.check_k(self.prompt_logprobs, "prompt_logprobs")
+
+
+@dataclass
+class Logprob:
+    """vLLM's Logprob: the log probability of a token, its rank (1 + the number of tokens with a larger logit), its text."""
+    logprob: float
+    rank: int = None
+    decoded_token: str = None
 
 
 @dataclass
@@ -37,6 +52,41 @@ class CompletionOutput:
     text: str
     token_ids: list
     finish_reason: str = None     # "stop" (EOS / stop id / stop string) or "length"
+    logprobs: list = None         # SamplingParams.logprobs: per kept token, {id: Logprob} of the token and its top-k
+    cumulative_logprob: float = None
+
+
+def logprob_dict(token, logprob, rank, top_ids, top_lps, tokenizer):
+    """{id: Logprob} of a token and its top-k (k or k + 1 entries).  A top-k entry's rank is 1 + the number of entries with a larger
+    logprob, all of which are in the top-k."""
+    d = {int(token): Logprob(float(logprob), int(rank), decode_text(tokenizer, [int(token)]))}
+    for i, lp in zip(top_ids, top_lps):
+        if int(i) >= 0 and int(i) not in d:
+            d[int(i)] = Logprob(float(lp), 1 + sum(1 for x in top_lps if x > lp), decode_text(tokenizer, [int(i)]))
+    return d
+
+
+def completion_logprobs(res, row, n_tokens, tokens, tokenizer):
+    """(logprobs, cumulative_logprob) of the first n_tokens generated tokens of ``row`` of a GenerationLogprobs."""
+    out = [logprob_dict(tokens[j], res.logprobs[row, j], res.ranks[row, j], res.top_ids[row, j], res.top_logprobs[row, j], tokenizer)
+           for j in range(n_tokens)]
+    return out, float(sum(float(res.logprobs[row, j]) for j in range(n_tokens)))
+
+
+def prompt_logprob_dicts(entries, tokenizer):
+    """RequestOutput.prompt_logprobs from GenerationLogprobs.prompt[row]: None, or {id: Logprob} of the token and its top-k."""
+    return [None if e is None else logprob_dict(e.token_id, e.logprob, e.rank, e.top_ids, e.top_logprobs, tokenizer) for e in entries]
+
+
+def tokens_before_stop_string(tokenizer, tokens, stops):
+    """The number of leading tokens whose text first contains a stop string (all of them when none does): the tokens the cut text
+    came from, the one that completed the stop string included."""
+    if not any(stops):
+        return len(tokens)
+    for n in range(1, len(tokens) + 1):
+        if cut_at_stop_string(decode_text(tokenizer, tokens[:n]), stops)[1]:
+            return n
+    return len(tokens)
 
 
 def eos_ids(config, stop_token_ids=None, extra=None):
@@ -103,6 +153,7 @@ class RequestOutput:
     prompt: str
     outputs: list
     num_cached_tokens: int = 0          # prompt positions (patch rows included) whose KV came from the prefix cache
+    prompt_logprobs: list = None        # SamplingParams.prompt_logprobs: per prompt token, None (the first) or {id: Logprob}
 
 
 def _free_port():
@@ -238,6 +289,8 @@ class LLM:
 
     def generate(self, inputs, sampling_params=None, use_tqdm=False, streamer=None):
         sp = sampling_params or SamplingParams()
+        if (sp.logprobs is not None or sp.prompt_logprobs is not None) and self.model.tp_size > 1:
+            raise ValueError("logprobs / prompt_logprobs are single-GPU only (tensor_parallel_size must be 1)")
         if isinstance(inputs, (dict, str)):
             inputs = [inputs]
         # plain strings are text-only prompts (llm_utils.py:127 passes a list of str to the same call)
@@ -247,8 +300,8 @@ class LLM:
             # n completions per request = n copies of the request in the batch, each row with its own draw
             # (llm_utils.py:127-130 reads outputs[i].outputs[j].text for j < n)
             flat = self._generate([r for r in inputs for _ in range(n)], sp)
-            return [RequestOutput(inputs[i]["prompt"], [flat[i * n + j].outputs[0] for j in range(n)], flat[i * n].num_cached_tokens)
-                    for i in range(len(inputs))]
+            return [RequestOutput(inputs[i]["prompt"], [flat[i * n + j].outputs[0] for j in range(n)], flat[i * n].num_cached_tokens,
+                                  flat[i * n].prompt_logprobs) for i in range(len(inputs))]
         return self._generate(inputs, sp, streamer)
 
     def _generate(self, inputs, sp, streamer=None):
@@ -278,14 +331,20 @@ class LLM:
                                       temperature=sp.temperature, top_p=sp.top_p, top_k=(sp.top_k if sp.top_k and sp.top_k > 0 else None),
                                       ignore_eos=sp.ignore_eos, seed=(None if sp.seed is None else sp.seed + i0),
                                       eos_token_id=stop_ids, streamer=streamer,
-                                      repetition_penalty=(sp.repetition_penalty if sp.repetition_penalty not in (None, 1.0) else None))
+                                      repetition_penalty=(sp.repetition_penalty if sp.repetition_penalty not in (None, 1.0) else None),
+                                      logprobs=sp.logprobs, prompt_logprobs=sp.prompt_logprobs)
+            res = self.model.last_logprobs if (sp.logprobs is not None or sp.prompt_logprobs is not None) else None
             for b, req in enumerate(chunk):
                 # a row ends at ITS first stop id (the batch-wide tail after it is the pad fill of generate())
                 toks, fin = cut_at_stop(ids[b, S:].tolist(), stop_ids, sp.ignore_eos)
                 text, hit = cut_at_stop_string(decode_text(self.tokenizer, toks), stops)
                 hits = getattr(self.model, "last_cached_positions", None)
-                outs.append(RequestOutput(req["prompt"], [CompletionOutput(text, toks, "stop" if hit else fin)],
-                                          int(hits[b]) if hits is not None else 0))
+                co = CompletionOutput(text, toks, "stop" if hit else fin)
+                if sp.logprobs is not None:
+                    keep = tokens_before_stop_string(self.tokenizer, toks, stops) if hit else len(toks)
+                    co.logprobs, co.cumulative_logprob = completion_logprobs(res, b, keep, toks, self.tokenizer)
+                plp = prompt_logprob_dicts(res.prompt[b], self.tokenizer) if sp.prompt_logprobs is not None else None
+                outs.append(RequestOutput(req["prompt"], [co], int(hits[b]) if hits is not None else 0, plp))
         return outs
 
 

@@ -217,6 +217,22 @@ int cts_sample_advance(cts_ctx* ctx, const void* logits, long long vocab, int ba
                        unsigned long long seed, int* out_tokens, int out_ld, int* step_ptr, int* cur_ids, int* positions,
                        int* seq_lens, int* slot_map, const int* page_table, int max_pages, int page_size, int dtype, void* stream);
 
+/* Log probabilities of `rows` rows of 16-bit logits [rows, ld] (vLLM's raw logprobs), in fp32 from the stored values:
+ *   lse = m + log sum_i exp(x_i - m);  chosen_logprob = x_c - lse;  chosen_rank = 1 + #{i : x_i > x_c};
+ *   the k (0..20) largest entries as (id, x_i - lse), by value descending, equal values by the smaller id.
+ * NaN logits take no part in m, the sum, the ranks or the top-k (-inf entries are allowed); a NaN chosen logit (or a chosen id
+ * outside [0, vocab)) gives a NaN logprob and rank 0; top-k slots past the row's non-NaN entries get id -1 and a NaN logprob.
+ * Column: col = step_ptr[0] - 1 (the column the preceding greedy / sample advance wrote) with a non-null step_ptr, else 0.
+ *   chosen id:     chosen[r * chosen_ld + col]            (chosen may be null when out_logprob and out_rank are)
+ *   outputs:       out_logprob / out_rank [r * out_ld + col], out_topk_ids / out_topk_logprobs [(r * out_ld + col) * k + j]
+ * Each row is split over ceil(vocab / 2048) CTAs merged by the last one to arrive; workspace holds
+ * cts_logprobs_workspace_floats(rows, vocab, k) floats (8-byte aligned), counters int[rows] zero-filled ONCE (the kernel resets
+ * them), so a launch can be captured in a CUDA graph.  vocab <= 2^24, ld >= vocab, rows <= 65535. */
+long long cts_logprobs_workspace_floats(int rows, long long vocab, int k);
+int cts_logprobs(cts_ctx* ctx, const void* logits, long long vocab, long long ld, int rows, const int* chosen, int chosen_ld,
+                 const int* step_ptr, int k, float* out_logprob, int* out_rank, int* out_topk_ids, float* out_topk_logprobs, int out_ld,
+                 float* workspace, int* counters, int dtype, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Tensor parallelism over NVLink peer memory (SURVEY.md §5, §8e; replaces RowParallelLinear's NCCL all-reduce +
  * residual add + RMSNorm, vllm qwen2.py:100-116,168-174,299-311, for decode-sized messages).

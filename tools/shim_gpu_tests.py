@@ -132,6 +132,12 @@ SELECT = {
     # other series under the same ids, and the engine's shared-prefix admissions
     "test_gpu_zz_h_prefix_cache.py": "(cold_call and tiny) or (warm_call and tiny-16-insert) or boundary_inside or (same_ids and tiny) "
                                      "or (continuous_engine and bf16)",
+    # log probabilities: the kernel at the small vocabularies (ties, non-finite entries, strides, column mode, argument errors), and
+    # generate() / the engine with logprobs on the tiny model
+    "test_gpu_logprobs.py": "(match_log_softmax and (1000 or 1003) and (-1- or -5-)) or (row_stride and 1000) or (ties and 1003) "
+                            "or (column_mode and 1000) or argument_errors",
+    "test_gpu_zz_i_logprobs.py": "(decode_logprobs and tiny-bfloat16-default) or (prompt_logprobs and tiny-bf16) "
+                                 "or continuous_engine",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
