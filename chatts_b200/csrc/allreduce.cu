@@ -180,6 +180,9 @@ peer_allreduce_residual_rmsnorm_kernel(const float* __restrict__ local_part, int
 // (largest value, lowest index on ties -- identical on every rank) and advances the device-side decode state.
 // Replaces "ParallelLMHead logits all-gather + sampler" (chatts_vllm.py:607-610) for greedy decoding, which lets a
 // tensor-parallel decode step be captured in one CUDA graph.  One CTA per sequence.
+// The token is what cts_greedy_advance picks from the whole row: the smallest index holding the maximum over the non-NaN
+// entries, or token 0 when no entry is greater than -inf (all -inf / NaN).  A shard without such an entry publishes
+// (-inf, 0x7fffffff), which loses to any real candidate and which the merge maps to token 0 when every shard is empty.
 template <typename T>
 __global__ void __launch_bounds__(1024)
 peer_greedy_advance_kernel(const T* __restrict__ logits, long long vshard, int rank, int world, float2* const* __restrict__ peer_cand,
@@ -220,7 +223,7 @@ peer_greedy_advance_kernel(const T* __restrict__ logits, long long vshard, int r
       if (ob > best || (ob == best && oi < best_i)) { best = ob; best_i = oi; }
     }
     // push my candidate to every rank (slot [rank][b]) and then the flag
-    const float gidx = __int_as_float((int)(best_i + (long long)rank * vshard));
+    const float gidx = __int_as_float(best_i < vshard ? (int)(best_i + (long long)rank * vshard) : 0x7fffffff);
     if (lane < world) {
       float2* dst = peer_cand[lane] + (long long)rank * max_b + b;
       asm volatile("st.relaxed.sys.global.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(best), "f"(gidx) : "memory");

@@ -1,7 +1,9 @@
 """Tensor-parallel plumbing: symmetric (cudaIpc) buffers shared by the ranks of one NVSwitch domain.
 
 torch.distributed carries only the 64-byte IPC handles (and NCCL the large prefill all-reduces); the decode
-all-reduce itself is cts_peer_allreduce_residual_rmsnorm over the mapped peer pointers."""
+all-reduces run over the mapped peer pointers.  By default that is cts_peer_allreduce_ll, the two-shot kernel with its
+flags inside the data; CTS_PEER_LL=0 selects cts_peer_allreduce_residual_rmsnorm, the one-shot kernel that pushes every
+rank's rows to every peer.  Greedy decoding takes the global argmax with cts_peer_greedy_advance over the candidate tables."""
 
 import torch
 import torch.distributed as dist

@@ -138,6 +138,9 @@ SELECT = {
                             "or (column_mode and 1000) or argument_errors",
     "test_gpu_zz_i_logprobs.py": "(decode_logprobs and tiny-bfloat16-default) or (prompt_logprobs and tiny-bf16) "
                                  "or continuous_engine",
+    # the tensor-parallel kernels with one rank (a rank waits only on itself): the vocab-parallel greedy step against
+    # cts_greedy_advance, the one-shot all-reduce at every cluster width, and both kernels' argument errors
+    "test_gpu_zz_j_peer_tp.py": "(W1 and not 38016 and not 76032 and not 32768) or rejects_bad_arguments",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
