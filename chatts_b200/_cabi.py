@@ -33,6 +33,7 @@ SYMBOLS = [
     "cts_rep_penalty_mark", "cts_rep_penalty_apply", "cts_gemm_w4", "cts_gemm_w4_suggest_split", "cts_gemm_w4_mma", "cts_gemm_w4_mma_suggest_split",
     "cts_gemm_fp8", "cts_gemm_fp8_suggest_split", "cts_fp8_dequant", "cts_attn_prefill_paged",
     "cts_logprobs_workspace_floats", "cts_logprobs",
+    "cts_struct_mask_build", "cts_struct_mask_apply", "cts_struct_advance",
 ]
 LOGPROBS_MAX_K = 20
 FUSED_RESIDUAL, FUSED_SWIGLU, FUSED_QKV_ROPE = 0, 1, 2
@@ -202,6 +203,11 @@ def load_library():
     lib.cts_logprobs_workspace_floats.restype = ll
     lib.cts_logprobs.argtypes = [vp, vp, ll, ll, i, vp, i, vp, i, vp, vp, vp, vp, i, vp, vp, i, vp]
     lib.cts_logprobs.restype = i
+    lib.cts_struct_mask_build.argtypes = [vp, vp, vp, i, vp, vp, ll, vp, i, vp, i, vp]
+    lib.cts_struct_mask_apply.argtypes = [vp, vp, ll, ll, i, vp, vp, i, i, vp]
+    lib.cts_struct_advance.argtypes = [vp, vp, i, vp, vp, vp, vp, ll, vp, i, vp]
+    for name in ("cts_struct_mask_build", "cts_struct_mask_apply", "cts_struct_advance"):
+        getattr(lib, name).restype = i
     # ---- A9: LoRA fine-tune step
     lib.cts_attn_prefill_lse.argtypes = [vp, vp, vp, vp, vp, i, i, ll, i, i, i, f, vp, vp, i, vp]
     lib.cts_attn_bwd.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i, i, ll, i, i, i, f, vp, vp, vp, vp, i, vp]
@@ -609,6 +615,26 @@ class Context:
     def rep_penalty_apply(self, logits, batch, seen, penalty):
         self._chk(self.lib.cts_rep_penalty_apply(self.h, _p(logits), logits.shape[-1], logits.stride(0), batch, _p(seen), seen.shape[1],
                                                  float(penalty), dtype_code(logits.dtype), _stream()))
+
+    def struct_mask_build(self, trans, accept, offsets, token_bytes, stop_ids, allowed):
+        """allowed int32 [S, ceil(V / 32)] from the DFA trans int32 [S, 256] / accept uint8 [S], the token bytes (offsets int64 [V + 1],
+        token_bytes uint8) and stop_ids int32 [n] (cts_struct_mask_build)."""
+        n = stop_ids.numel()
+        self._chk(self.lib.cts_struct_mask_build(self.h, _p(trans), _p(accept), trans.shape[0], _p(offsets), _p(token_bytes),
+                                                 offsets.numel() - 1, _p(stop_ids) if n else None, n, _p(allowed), allowed.shape[1],
+                                                 _stream()))
+
+    def struct_mask_apply(self, logits, batch, state, allowed, vocab=None):
+        """logits[b, i] = -inf where bit i of allowed[state[b]] is clear; rows with state[b] < 0 untouched (cts_struct_mask_apply)."""
+        vocab = logits.shape[-1] if vocab is None else vocab
+        self._chk(self.lib.cts_struct_mask_apply(self.h, _p(logits), int(vocab), logits.stride(0), int(batch), _p(state), _p(allowed),
+                                                 allowed.shape[1], dtype_code(logits.dtype), _stream()))
+
+    def struct_advance(self, cur_ids, batch, state, trans, offsets, token_bytes, stop_ids):
+        """state[b] <- the DFA state reached by walking the bytes of cur_ids[b] (cts_struct_advance)."""
+        n = stop_ids.numel()
+        self._chk(self.lib.cts_struct_advance(self.h, _p(cur_ids), int(batch), _p(state), _p(trans), _p(offsets), _p(token_bytes),
+                                              offsets.numel() - 1, _p(stop_ids) if n else None, n, _stream()))
 
     # ------------------------------------------------------------------ A9: LoRA fine-tune step
     def attn_prefill_lse(self, q, k, v, cu_seqlens, batch, max_seqlen, nh, nkv, head_dim, scale, out, lse):

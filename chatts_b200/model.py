@@ -17,7 +17,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from . import _cabi, layout, prefix_cache
+from . import _cabi, layout, prefix_cache, structured
 from . import logprobs as lpmod
 from .trace import span
 from ._cabi import EPI_NONE, EPI_PARTIAL_F32, EPI_RESIDUAL, EPI_SWIGLU_IL
@@ -1097,7 +1097,7 @@ class ChatTSForCausalLM:
     def generate(self, input_ids=None, attention_mask=None, timeseries=None, max_new_tokens=None, max_length=None,
                  do_sample=None, temperature=None, top_p=None, top_k=None, streamer=None, eos_token_id=None, pad_token_id=None,
                  synced_gpus=False, sync_every=16, ignore_eos=False, seed=None, repetition_penalty=None, logprobs=None,
-                 prompt_logprobs=None, **_):
+                 prompt_logprobs=None, structured_outputs=None, tokenizer=None, **_):
         """model.generate(**processor_out, max_new_tokens=...) -> LongTensor [B, S + new] whose first S columns are
         the ORIGINAL (un-expanded) input ids (README.md:102-103).
 
@@ -1106,11 +1106,23 @@ class ChatTSForCausalLM:
         (chatts_b200.logprobs.GenerationLogprobs; None when neither was asked).  They describe the distribution the token was picked
         from: log_softmax in fp32 of the logits, after the repetition penalty when one is set and before temperature, top-k and top-p
         (vLLM's raw logprobs whenever repetition_penalty == 1).  A call with prompt_logprobs computes every prompt position (no
-        prefix-cache hits; its pages are still indexed).  Single GPU only."""
+        prefix-cache hits; its pages are still indexed).  Single GPU only.
+
+        structured_outputs = StructuredOutputsParams or {"choice": [...]} / {"regex": "..."}: every row's output is one of the choices,
+        or a full match of the regex (chatts_b200.structured), with ``tokenizer`` giving the bytes of each token id (None: ids < 256 are
+        bytes, as SimpleTokenizer encodes).  Each step, the logits of the tokens the automaton does not allow become -inf before the
+        repetition penalty and the greedy or sampled pick, and the logprobs describe that masked distribution; the stop ids are allowed
+        exactly where the output is complete.  If max_new_tokens runs out first, the output is cut there.  Not with ignore_eos; single
+        GPU only."""
         cfg, dev = self.config, self.device
         lpk, plk = lpmod.check_k(logprobs, "logprobs"), lpmod.check_k(prompt_logprobs, "prompt_logprobs")
         if (lpk is not None or plk is not None) and self.tp_size > 1:
             raise ValueError("logprobs / prompt_logprobs are single-GPU only (tensor_parallel_size must be 1)")
+        so = structured.resolve(structured_outputs)
+        if so is not None and self.tp_size > 1:
+            raise ValueError("structured_outputs are single-GPU only (tensor_parallel_size must be 1)")
+        if so is not None and ignore_eos:
+            raise ValueError("structured_outputs end the output with a stop id: they cannot be combined with ignore_eos")
         self.last_logprobs = None
         gd = getattr(self, "generation_defaults", None)
         if gd:                                          # checkpoint defaults apply only where the caller said nothing
@@ -1137,6 +1149,12 @@ class ChatTSForCausalLM:
         eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
         eos_set = set(eos) if isinstance(eos, (list, tuple, set)) else {int(eos)}
         pad = cfg.pad_token_id if pad_token_id is None else pad_token_id
+        auto = None
+        if so is not None:
+            # compiled (or found in the cache) before any page is taken: a pattern error leaves the pool as it was
+            if getattr(self, "_struct_cache", None) is None:
+                self._struct_cache = structured.AutomatonCache(self.ctx, dev)
+            auto = self._struct_cache.get(so, tokenizer, self.config.vocab_size, eos_set)
         if do_sample and temperature is None:
             temperature = 1.0                                   # HF GenerationConfig default when do_sample=True names no temperature
         greedy = not (do_sample and temperature > 0)
@@ -1167,6 +1185,12 @@ class ChatTSForCausalLM:
             if seed is not None:
                 gen.manual_seed(int(seed))
             kseed = int(seed) if seed is not None else 0
+            # structured outputs: each row's automaton state lives on the device next to cur_ids; every step masks the logits by it
+            # before anything reads them and walks it over the picked token after the advance
+            struct_state = None
+            if auto is not None:
+                struct_state = torch.zeros(B, dtype=torch.int32, device=dev)
+                auto.mask_apply(self.ctx, logits, B, struct_state)
 
             def sample(lg, step):
                 if self.use_sample_kernel:
@@ -1199,6 +1223,8 @@ class ChatTSForCausalLM:
                     sample(lg, step)
                 if seen is not None:
                     self.ctx.rep_penalty_mark(st.cur_ids, None, seen, self.config.vocab_size)
+                if auto is not None:
+                    auto.advance(self.ctx, st.cur_ids, B, struct_state)
 
             # logprobs: one cts_logprobs launch after each advance, over the logits the token was picked from; the kernel advances
             # (greedy, sample) leave step_ptr one past the column they wrote, the torch sampler does not move it.  Only called when
@@ -1234,10 +1260,12 @@ class ChatTSForCausalLM:
                     if produced >= max_new_tokens or done.all():
                         break
                 with span("cts.decode_step"):
-                    if greedy and seen is None:
+                    if greedy and seen is None and auto is None:
                         self._decode_step(st, sample=True)
                     else:
                         self._decode_step(st, sample=False)
+                        if auto is not None:
+                            auto.mask_apply(self.ctx, st.full_logits, B, struct_state)
                         if seen is not None:
                             self.ctx.rep_penalty_apply(st.full_logits, B, seen, rep)
                         advance(st.full_logits, produced)
@@ -1255,6 +1283,9 @@ class ChatTSForCausalLM:
             res = lpmod.GenerationLogprobs()
             if lpb is not None:
                 res.logprobs, res.ranks, res.top_ids, res.top_logprobs = lpb.host(n_out)
+                if auto is not None:                      # a token the constraint refused has probability 0: an empty top-k slot
+                    gone = np.isneginf(res.top_logprobs)
+                    res.top_ids[gone], res.top_logprobs[gone] = -1, np.nan
             if plp is not None:
                 tgt, rows, cols, pbuf = plp
                 res.prompt = lpmod.prompt_entries(ids_cpu, am_cpu, rows, cols, tgt, *(a[:, 0] for a in pbuf.host(1)))

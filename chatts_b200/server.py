@@ -23,6 +23,7 @@ from concurrent.futures import Future
 from dataclasses import dataclass, field
 
 from .logprobs import check_k
+from .structured import compile_params, resolve as resolve_structured
 from .vllm_compat import IncrementalDecoder, decode_text, eos_ids
 
 MAX_TS_DEFAULT = 15          # scripts/start_vllm_server.sh:9  (--limit-mm-per-prompt timeseries=15)
@@ -89,6 +90,9 @@ class Engine:
             raise ValueError(f"at most {self.max_ts} time series per prompt")
         if self.scheduler == "continuous" and params.get("temperature", 0.0) > 0:
             raise ValueError("the continuous scheduler decodes greedily; start the server with --scheduler batch for sampling")
+        if self.scheduler == "continuous" and params.get("structured_outputs") is not None:
+            raise ValueError("the continuous scheduler does not constrain outputs; start the server with --scheduler batch for "
+                             "structured_outputs")
         job = _Job(prompt, list(series), dict(params), stream_q=queue.Queue() if stream else None)
         self.q.put(job)
         return job
@@ -258,9 +262,28 @@ class _QueueStreamer:
             self.q.put(tail)
 
 
+def _structured_from_body(body):
+    """The constraint of a request body as a dict of StructuredOutputsParams fields (None without one): vLLM's ``structured_outputs``
+    object, or its older ``guided_choice`` / ``guided_regex`` fields.  The pattern is compiled here, so a bad one is a 400."""
+    spec = body.get("structured_outputs")
+    guided = {k: body[f"guided_{k}"] for k in ("choice", "regex") if body.get(f"guided_{k}") is not None}
+    if spec is not None and guided:
+        raise ValueError("send either structured_outputs or guided_choice / guided_regex, not both")
+    if spec is None:
+        spec = guided or None
+    if spec is not None and not isinstance(spec, dict):
+        raise ValueError("structured_outputs must be an object")
+    so = resolve_structured(spec)
+    if so is None:
+        return None
+    compile_params(so)
+    return {"choice": list(so.choice)} if so.choice is not None else {"regex": so.regex}
+
+
 def _sampling_from_body(body, chat=False):
     """SamplingParams fields of an OpenAI request body.  Log probabilities: chat takes ``logprobs: true`` with ``top_logprobs`` 0..20,
-    completions ``logprobs: <int>`` 0..20; neither works with ``stream`` (ValueError, a 400 for the client)."""
+    completions ``logprobs: <int>`` 0..20; neither works with ``stream`` (ValueError, a 400 for the client).  Constraints:
+    ``structured_outputs`` ({"choice": [...]} or {"regex": "..."}) or ``guided_choice`` / ``guided_regex``."""
     p = {"max_tokens": int(body.get("max_tokens") or body.get("max_completion_tokens") or 256),
          "temperature": float(body.get("temperature", 0.0) or 0.0), "top_p": float(body.get("top_p", 1.0) or 1.0),
          "top_k": int(body.get("top_k", 0) or 0), "n": int(body.get("n", 1) or 1)}
@@ -287,6 +310,11 @@ def _sampling_from_body(body, chat=False):
         p["logprobs"] = check_k(k, "top_logprobs" if chat else "logprobs")
         if body.get("stream"):
             raise ValueError("logprobs are not available on streamed responses: send the request with stream=false")
+    so = _structured_from_body(body)
+    if so is not None:
+        if p.get("ignore_eos"):
+            raise ValueError("structured_outputs end the output with a stop id: they cannot be combined with ignore_eos")
+        p["structured_outputs"] = so
     return p
 
 

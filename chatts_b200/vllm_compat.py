@@ -13,6 +13,7 @@ from . import logprobs as lpmod
 from .config import ChatTSConfig
 from .model import ChatTSForCausalLM
 from .processor import ChatTSProcessor, SimpleTokenizer
+from .structured import StructuredOutputsParams, resolve as _resolve_structured  # noqa: F401  (StructuredOutputsParams is public here)
 
 MAX_TS_PER_PROMPT = 50      # chatts_vllm.py:219-220
 
@@ -33,10 +34,14 @@ class SamplingParams:
     repetition_penalty: float = 1.0                   # vLLM SamplingParams.repetition_penalty (prompt + generated tokens)
     logprobs: int = None                              # 0..20: logprob of every generated token plus its top-k (single GPU)
     prompt_logprobs: int = None                       # 0..20: the same for every prompt token after the first (single GPU)
+    structured_outputs: StructuredOutputsParams = None  # choice / regex constraint on the output (a dict of its fields is accepted)
 
     def __post_init__(self):
         lpmod.check_k(self.logprobs, "logprobs")
         lpmod.check_k(self.prompt_logprobs, "prompt_logprobs")
+        self.structured_outputs = _resolve_structured(self.structured_outputs)
+        if self.structured_outputs is not None and self.ignore_eos:
+            raise ValueError("structured_outputs end the output with a stop id: they cannot be combined with ignore_eos")
 
 
 @dataclass
@@ -291,6 +296,8 @@ class LLM:
         sp = sampling_params or SamplingParams()
         if (sp.logprobs is not None or sp.prompt_logprobs is not None) and self.model.tp_size > 1:
             raise ValueError("logprobs / prompt_logprobs are single-GPU only (tensor_parallel_size must be 1)")
+        if sp.structured_outputs is not None and self.model.tp_size > 1:
+            raise ValueError("structured_outputs are single-GPU only (tensor_parallel_size must be 1)")
         if isinstance(inputs, (dict, str)):
             inputs = [inputs]
         # plain strings are text-only prompts (llm_utils.py:127 passes a list of str to the same call)
@@ -332,7 +339,8 @@ class LLM:
                                       ignore_eos=sp.ignore_eos, seed=(None if sp.seed is None else sp.seed + i0),
                                       eos_token_id=stop_ids, streamer=streamer,
                                       repetition_penalty=(sp.repetition_penalty if sp.repetition_penalty not in (None, 1.0) else None),
-                                      logprobs=sp.logprobs, prompt_logprobs=sp.prompt_logprobs)
+                                      logprobs=sp.logprobs, prompt_logprobs=sp.prompt_logprobs,
+                                      structured_outputs=sp.structured_outputs, tokenizer=self.tokenizer)
             res = self.model.last_logprobs if (sp.logprobs is not None or sp.prompt_logprobs is not None) else None
             for b, req in enumerate(chunk):
                 # a row ends at ITS first stop id (the batch-wide tail after it is the pad fill of generate())

@@ -595,6 +595,25 @@ int cts_rep_penalty_mark(cts_ctx* ctx, const int* tokens, const int* rows, int n
 int cts_rep_penalty_apply(cts_ctx* ctx, void* logits, long long vocab, long long ld, int batch, const unsigned* seen, int words_per_row,
                           float penalty, int dtype, void* stream);
 
+/* Structured outputs (csrc/structured.cu): decoding constrained by a byte DFA (chatts_b200/structured.py compiles a choice list or a
+ * regex into it), the automaton's per-row state kept on the device so a constrained step makes no host round trip.
+ *   trans      int [S, 256]: next state of (state, byte), -1 where undefined; accept uint8 [S]
+ *   offsets    int64 [vocab + 1], bytes uint8: the bytes of token t are bytes[offsets[t] .. offsets[t + 1]) (none: never allowed)
+ *   stop_ids   int [n_stop] (n_stop <= 64): allowed exactly in accepting states; choosing one leaves the state unchanged
+ *   allowed    uint32 [S, words_per_state], words_per_state = ceil(vocab / 32): bit t of row s = token t allowed in state s
+ * cts_struct_mask_build: token t is allowed in state s iff walking its bytes from s never meets an undefined transition.
+ * cts_struct_mask_apply: logits[b * ld + i] = -inf where bit i of allowed[state[b]] is clear; entries whose bit is set and rows
+ *   with state[b] < 0 are not written.
+ * cts_struct_advance: state[b] = the state reached by walking the bytes of cur_ids[b] from state[b] (run after the greedy / sample
+ *   advance wrote cur_ids); rows with state[b] < 0, stop ids and a token whose walk fails leave state[b] unchanged. */
+int cts_struct_mask_build(cts_ctx* ctx, const int* trans, const unsigned char* accept, int num_states, const long long* offsets,
+                          const unsigned char* bytes, long long vocab, const int* stop_ids, int n_stop, unsigned* allowed,
+                          int words_per_state, void* stream);
+int cts_struct_mask_apply(cts_ctx* ctx, void* logits, long long vocab, long long ld, int batch, const int* state,
+                          const unsigned* allowed, int words_per_state, int dtype, void* stream);
+int cts_struct_advance(cts_ctx* ctx, const int* cur_ids, int batch, int* state, const int* trans, const long long* offsets,
+                       const unsigned char* bytes, long long vocab, const int* stop_ids, int n_stop, void* stream);
+
 /* Debug / profiling aid (csrc/trace.cuh): instrumented kernels append {tag, %globaltimer} records to `buf` (unsigned long long
  * [2 + 2*capacity]: [0] cursor, [1] capacity, then the records) -- the overlapped timeline of a CUDA-graph replay that ncu, which
  * serialises kernels, cannot show (tools/trace_decode_step.py).  buf = NULL switches it off (the default). */
