@@ -34,6 +34,7 @@ SYMBOLS = [
     "cts_gemm_fp8", "cts_gemm_fp8_suggest_split", "cts_fp8_dequant", "cts_attn_prefill_paged",
     "cts_logprobs_workspace_floats", "cts_logprobs",
     "cts_struct_mask_build", "cts_struct_mask_apply", "cts_struct_advance",
+    "cts_beam_select", "cts_beam_fork_kv",
 ]
 LOGPROBS_MAX_K = 20
 FUSED_RESIDUAL, FUSED_SWIGLU, FUSED_QKV_ROPE = 0, 1, 2
@@ -207,6 +208,10 @@ def load_library():
     lib.cts_struct_mask_apply.argtypes = [vp, vp, ll, ll, i, vp, vp, i, i, vp]
     lib.cts_struct_advance.argtypes = [vp, vp, i, vp, vp, vp, vp, ll, vp, i, vp]
     for name in ("cts_struct_mask_build", "cts_struct_mask_apply", "cts_struct_advance"):
+        getattr(lib, name).restype = i
+    lib.cts_beam_select.argtypes = [vp, i, i, i, ll, vp, vp, vp, i, vp, i, i, f] + [vp] * 15 + [i, i, vp, vp]
+    lib.cts_beam_fork_kv.argtypes = [vp, vp, i, ll, i, i, i, vp, i, vp]
+    for name in ("cts_beam_select", "cts_beam_fork_kv"):
         getattr(lib, name).restype = i
     # ---- A9: LoRA fine-tune step
     lib.cts_attn_prefill_lse.argtypes = [vp, vp, vp, vp, vp, i, i, ll, i, i, i, f, vp, vp, i, vp]
@@ -635,6 +640,25 @@ class Context:
         n = stop_ids.numel()
         self._chk(self.lib.cts_struct_advance(self.h, _p(cur_ids), int(batch), _p(state), _p(trans), _p(offsets), _p(token_bytes),
                                               offsets.numel() - 1, _p(stop_ids) if n else None, n, _stream()))
+
+    def beam_select(self, batch, num_beams, keep, vocab, cand_ids, cand_logprobs, eos_ids, len_den, max_new, early_stopping,
+                    length_penalty, run_scores, fin_scores, fin_info, prompt_flags, step_ptr, bp_tokens, bp_parents, cur_ids, positions,
+                    seq_lens, slot_map, page_table, page_table_old, own_pages, spare_pages, page_size, fork):
+        """One beam-search selection step of ``batch`` prompts x ``num_beams`` rows (cts_beam_select; shapes in include/chatts_b200.h).
+        early_stopping: False, True or "never"; eos_ids int32 [n] (n may be 0)."""
+        es = {False: 0, True: 1, "never": 2}[early_stopping]
+        n = eos_ids.numel()
+        self._chk(self.lib.cts_beam_select(self.h, int(batch), int(num_beams), int(keep), int(vocab), _p(cand_ids), _p(cand_logprobs),
+                                           _p(eos_ids) if n else None, n, _p(len_den), int(max_new), es, float(length_penalty),
+                                           _p(run_scores), _p(fin_scores), _p(fin_info), _p(prompt_flags), _p(step_ptr), _p(bp_tokens),
+                                           _p(bp_parents), _p(cur_ids), _p(positions), _p(seq_lens), _p(slot_map), _p(page_table),
+                                           _p(page_table_old), _p(own_pages), _p(spare_pages), page_table.shape[1], int(page_size), _p(fork),
+                                           _stream()))
+
+    def beam_fork_kv(self, kv, fork, rows):
+        """Copy-on-write of the forked rows' partial tail pages in kv [L, 2, num_pages, nkv, page_size, d] (cts_beam_fork_kv)."""
+        L, _, P, nkv, ps, d = kv.shape
+        self._chk(self.lib.cts_beam_fork_kv(self.h, _p(kv), L, P, nkv, ps, d, _p(fork), int(rows), _stream()))
 
     # ------------------------------------------------------------------ A9: LoRA fine-tune step
     def attn_prefill_lse(self, q, k, v, cu_seqlens, batch, max_seqlen, nh, nkv, head_dim, scale, out, lse):

@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _cabi, layout, prefix_cache, structured
+from . import beam as beammod
 from . import logprobs as lpmod
 from .trace import span
 from ._cabi import EPI_NONE, EPI_PARTIAL_F32, EPI_RESIDUAL, EPI_SWIGLU_IL
@@ -865,13 +866,14 @@ class ChatTSForCausalLM:
                     cached_pages=len(pool.page_of) if self.enable_prefix_caching else 0,
                     evictions=pool.evictions if self.enable_prefix_caching else 0)
 
-    def _alloc_prompt(self, lay, timeseries, extra, lookup=True):
+    def _alloc_prompt(self, lay, timeseries, extra, lookup=True, spare=0):
         """Pages for the prompts of ``lay`` plus ``extra`` decode positions each: (page_tables, held, keys, cached).  With prefix
         caching on, the leading full pages an earlier prefill indexed are shared (cached = positions per sequence they hold) and keys
         are what _prefix_register indexes once the prefill is enqueued; off, keys and cached are None.  lookup=False: no page is
-        shared (every position is computed), the keys are still returned for indexing."""
+        shared (every position is computed), the keys are still returned for indexing.  ``spare`` more pages, in no page table, are
+        taken in the same all-or-nothing check and are the last ``spare`` entries of held."""
         if not self.enable_prefix_caching:
-            return self._alloc_pages(lay.lens, extra) + (None, None)
+            return self._alloc_pages(lay.lens, extra, spare) + (None, None)
         cnt = self._host_counts[1].numpy() if lay.row_map.shape[0] > 0 else np.zeros(0, dtype=np.int64)
         seed = prefix_cache.chain_seed(self._merge_mode(), self.page_size, self._prefix_epoch)
         keys = prefix_cache.page_keys(lay, prefix_cache.series_digests(timeseries) if cnt.shape[0] else [], cnt, seed, self.page_size)
@@ -879,7 +881,7 @@ class ChatTSForCausalLM:
         pool, ps = self.pool, self.page_size
         hits = [pool.lookup(keys[b][: (int(n) - 1) // ps]) if lookup else [] for b, n in enumerate(lay.lens)]
         hit_set = {p for h in hits for p in h}
-        new = sum(n - len(h) for n, h in zip(needs, hits))
+        new = sum(n - len(h) for n, h in zip(needs, hits)) + spare
         # all-or-nothing: hits + free + evictable (minus the evictable pages this batch hits) against the need, before any reference
         avail = len(pool.free) + sum(1 for p in pool.evictable if p not in hit_set)
         if new > avail:
@@ -892,6 +894,7 @@ class ChatTSForCausalLM:
             pages = h + pool.alloc(n - len(h))
             pt[b, :n] = pages
             held += pages
+        held += pool.alloc(spare)
         cached = np.array([len(h) * ps for h in hits], dtype=np.int64)
         self._prefix_queried += int(lay.lens.sum())
         self._prefix_hits += int(cached.sum())
@@ -948,19 +951,20 @@ class ChatTSForCausalLM:
             needs.append(need)
         return needs
 
-    def _alloc_pages(self, lens, extra):
+    def _alloc_pages(self, lens, extra, spare=0):
         needs = self._page_needs(lens, extra)
         pt = np.zeros((len(needs), self.max_pages), dtype=np.int32)
         # all-or-nothing: every need is checked before the first page leaves the pool, so a failure can never strand pages
         # (ContinuousEngine._admit retries a RuntimeError; a leak there would shrink the pool for good)
-        if sum(needs) > self.pool.available():
-            raise RuntimeError(f"KV cache exhausted: need {sum(needs)} pages, {self.pool.available()} free of {self.pool.num_pages}")
+        if sum(needs) + spare > self.pool.available():
+            raise RuntimeError(f"KV cache exhausted: need {sum(needs) + spare} pages, {self.pool.available()} free of {self.pool.num_pages}")
         held = []
         try:
             for b, need in enumerate(needs):
                 pg = self.pool.alloc(need)
                 held += pg
                 pt[b, :need] = pg
+            held += self.pool.alloc(spare)
         except BaseException:
             self.pool.release(held)
             raise
@@ -1097,7 +1101,8 @@ class ChatTSForCausalLM:
     def generate(self, input_ids=None, attention_mask=None, timeseries=None, max_new_tokens=None, max_length=None,
                  do_sample=None, temperature=None, top_p=None, top_k=None, streamer=None, eos_token_id=None, pad_token_id=None,
                  synced_gpus=False, sync_every=16, ignore_eos=False, seed=None, repetition_penalty=None, logprobs=None,
-                 prompt_logprobs=None, structured_outputs=None, tokenizer=None, **_):
+                 prompt_logprobs=None, structured_outputs=None, tokenizer=None, num_beams=None, length_penalty=1.0, early_stopping=False,
+                 num_return_sequences=1, num_beam_groups=None, diversity_penalty=None, **_):
         """model.generate(**processor_out, max_new_tokens=...) -> LongTensor [B, S + new] whose first S columns are
         the ORIGINAL (un-expanded) input ids (README.md:102-103).
 
@@ -1113,7 +1118,13 @@ class ChatTSForCausalLM:
         bytes, as SimpleTokenizer encodes).  Each step, the logits of the tokens the automaton does not allow become -inf before the
         repetition penalty and the greedy or sampled pick, and the logprobs describe that masked distribution; the stop ids are allowed
         exactly where the output is complete.  If max_new_tokens runs out first, the output is cut there.  Not with ignore_eos; single
-        GPU only."""
+        GPU only.
+
+        num_beams > 1: beam search with transformers' semantics (chatts_b200.beam), ``length_penalty``, ``early_stopping`` (True, False or
+        "never") and ``num_return_sequences`` (<= num_beams) as there.  Returns [B * num_return_sequences, S + n], each prompt's best
+        hypotheses first, padded with pad_token_id; ``self.last_beam_scores`` holds their scores (transformers' sequences_scores, fp32),
+        and is None after any other call.  Greedy only (do_sample, repetition_penalty != 1, logprobs, structured outputs, a streamer
+        and tensor parallelism are refused with ValueError), and max(2, 1 + number of EOS ids) * num_beams <= 20."""
         cfg, dev = self.config, self.device
         lpk, plk = lpmod.check_k(logprobs, "logprobs"), lpmod.check_k(prompt_logprobs, "prompt_logprobs")
         if (lpk is not None or plk is not None) and self.tp_size > 1:
@@ -1139,6 +1150,19 @@ class ChatTSForCausalLM:
                 max_new_tokens = gd["max_new_tokens"]
             if repetition_penalty is None and gd.get("repetition_penalty") is not None:
                 repetition_penalty = gd["repetition_penalty"]
+        self.last_beam_scores = None
+        if num_beams not in (None, 1):
+            eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
+            eos_ids = [] if ignore_eos else sorted({int(e) for e in (eos if isinstance(eos, (list, tuple, set)) else [eos])})
+            shape = torch.as_tensor(input_ids).shape
+            B = int(shape[0]) if len(shape) > 1 else 1
+            keep = beammod.check_args(num_beams, length_penalty, early_stopping, num_return_sequences, len(eos_ids), B, self.max_batch,
+                                      do_sample=do_sample, num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty,
+                                      repetition_penalty=repetition_penalty, logprobs=logprobs, prompt_logprobs=prompt_logprobs,
+                                      structured_outputs=structured_outputs, streamer=streamer, tp_size=self.tp_size)
+            return self._beam_generate(input_ids, attention_mask, timeseries, max_new_tokens, max_length, eos_ids,
+                                       cfg.pad_token_id if pad_token_id is None else pad_token_id, int(num_beams), keep, length_penalty,
+                                       early_stopping, int(num_return_sequences), sync_every)
         ids_cpu, am_cpu, counts, lay = self._prepare_inputs(input_ids, attention_mask, timeseries)
         B, S = ids_cpu.shape
         if max_new_tokens is None:
@@ -1291,6 +1315,92 @@ class ChatTSForCausalLM:
                 res.prompt = lpmod.prompt_entries(ids_cpu, am_cpu, rows, cols, tgt, *(a[:, 0] for a in pbuf.host(1)))
             self.last_logprobs = res
         return torch.cat([torch.as_tensor(ids_cpu, dtype=torch.long), torch.as_tensor(out[:, :n_out])], dim=1)
+
+    def _beam_generate(self, input_ids, attention_mask, timeseries, max_new_tokens, max_length, eos_ids, pad, nb, keep, length_penalty,
+                       early_stopping, nrs, sync_every):
+        """Beam search (see generate): one prefill per prompt, then every step the decode step of the B * nb beam rows (graph replay
+        without the advance), cts_logprobs for each row's top ``keep`` candidates, cts_beam_select and cts_beam_fork_kv, all on one
+        stream; the host reads the per-prompt done flags every ``sync_every`` steps and walks the back-pointers once at the end."""
+        c, dev, ps = self.ctx, self.device, self.page_size
+        ids_cpu, am_cpu, counts, lay = self._prepare_inputs(input_ids, attention_mask, timeseries)
+        B, S = ids_cpu.shape
+        if max_new_tokens is None:
+            max_new_tokens = (max_length - S) if max_length is not None else 20
+        max_new = int(max_new_tokens)
+        if max_new <= 0:
+            return torch.as_tensor(ids_cpu, dtype=torch.long).repeat_interleave(nrs, 0)
+        R, V = B * nb, self.config.vocab_size
+        needs = self._page_needs(lay.lens, max_new)
+        n_extra = beammod.extra_pages(lay.lens, needs, nb, ps)
+        page_tables, held, keys, cached = self._alloc_prompt(lay, timeseries, max_new, spare=n_extra)
+        try:
+            table, own, spare = beammod.page_plan(page_tables, lay.lens, needs, nb, ps, held[len(held) - n_extra:])
+            with span("cts.prefill"):
+                logits = self._prefill(lay, counts, timeseries, page_tables, cached=cached)
+            self._prefix_register(keys, page_tables, lay.lens, cached)
+            self.last_cached_positions = cached
+            st = self._decode_state(R, max_new)
+            lens = np.repeat(lay.lens.astype(np.int32), nb)
+            run = np.zeros((B, nb), dtype=np.float32)
+            run[:, 1:] = -1e9
+            eos_arr = np.asarray(eos_ids, dtype=np.int32)
+            ints = np.concatenate([table.reshape(-1), own.reshape(-1), spare, lens - 1, lens, eos_arr]).astype(np.int32)
+            d_int = torch.from_numpy(ints).pin_memory().to(dev, non_blocking=True)
+            o = 0
+
+            def take(n):
+                nonlocal o
+                o += n
+                return d_int[o - n:o]
+            st.page_table.copy_(take(R * self.max_pages).view(R, self.max_pages))
+            own_d, spare_d = take(R * self.max_pages), take(R)
+            st.positions.copy_(take(R))                              # advanced to len by step 0's selection
+            st.seq_lens.copy_(take(R))
+            eos_d = take(len(eos_ids))
+            floats = np.concatenate([run.reshape(-1), np.full(R, -1e9, dtype=np.float32), beammod.len_den(max_new, length_penalty)])
+            d_f = torch.from_numpy(floats).pin_memory().to(dev, non_blocking=True)
+            run_d, fin_scores, den_d = d_f[:R], d_f[R:2 * R], d_f[2 * R:]
+            fin_info = torch.zeros(R, 4, dtype=torch.int32, device=dev)
+            flags = torch.zeros(B, 2, dtype=torch.int32, device=dev)
+            flags[:, 0] = 1                                          # early-stop heuristic unsatisfied, not done
+            bstep = torch.zeros(2, dtype=torch.int32, device=dev)
+            bp_tok = torch.zeros(max_new, R, dtype=torch.int32, device=dev)
+            bp_par = torch.zeros(max_new, R, dtype=torch.int32, device=dev)
+            table_old = torch.zeros_like(st.page_table)
+            fork = torch.zeros(R, 3, dtype=torch.int32, device=dev)
+            cand_ids = torch.zeros(R, 1, keep, dtype=torch.int32, device=dev)
+            cand_lp = torch.zeros(R, 1, keep, dtype=torch.float32, device=dev)
+            lp_ws = torch.empty(max(c.logprobs_workspace_floats(R, V, keep), 2), dtype=torch.float32, device=dev)
+            lp_cnt = torch.zeros(R, dtype=torch.int32, device=dev)
+
+            def select(lg):
+                c.logprobs(lg, R, None, keep, None, None, cand_ids, cand_lp, lp_ws, lp_cnt, vocab=V)
+                c.beam_select(B, nb, keep, V, cand_ids, cand_lp, eos_d, den_d, max_new, early_stopping, length_penalty, run_d,
+                              fin_scores, fin_info, flags, bstep, bp_tok, bp_par, st.cur_ids, st.positions, st.seq_lens, st.slot_map,
+                              st.page_table, table_old, own_d, spare_d, ps, fork)
+                c.beam_fork_kv(self.kv, fork, R)
+
+            select(logits[:, :V].repeat_interleave(nb, 0))          # step 0: every beam row sees its prompt's prefill logits
+            produced, chunk = 1, max(1, int(sync_every))
+            while produced < max_new:
+                if produced % chunk == 0 and bool(flags[:, 1].all()):
+                    break
+                with span("cts.decode_step"):
+                    self._decode_step(st, sample=False)
+                    select(st.full_logits)
+                produced += 1
+            toks, pars = bp_tok[:produced].cpu().numpy(), bp_par[:produced].cpu().numpy()
+            scores, info = fin_scores.cpu().numpy(), fin_info.cpu().numpy()
+        finally:
+            self.pool.release(held)
+        hyps = [beammod.hypothesis(toks, pars, info[b * nb + i]) for b in range(B) for i in range(nrs)]
+        n = max(max(len(h) for h in hyps), 1)
+        out = np.full((B * nrs, S + n), pad, dtype=np.int64)
+        out[:, :S] = np.repeat(ids_cpu, nrs, axis=0)
+        for r, h in enumerate(hyps):
+            out[r, S:S + len(h)] = h
+        self.last_beam_scores = torch.from_numpy(np.stack([scores[b * nb:b * nb + nrs] for b in range(B)]).reshape(-1).copy())
+        return torch.from_numpy(out)
 
     def _sample_advance(self, st, logits, step, temperature, top_p, gen, top_k=None):
         """Stochastic sampling (temperature / top-p, chatts/utils/inference_tsmllm_deepspeed.py:95-100).  Round 1: the

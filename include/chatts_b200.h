@@ -614,6 +614,41 @@ int cts_struct_mask_apply(cts_ctx* ctx, void* logits, long long vocab, long long
 int cts_struct_advance(cts_ctx* ctx, const int* cur_ids, int batch, int* state, const int* trans, const long long* offsets,
                        const unsigned char* bytes, long long vocab, const int* stop_ids, int n_stop, void* stream);
 
+/* Beam search (csrc/beam.cu): transformers' GenerationMixin._beam_search with the beams kept on the device.  A step is four launches on
+ * one stream: the decode step of the batch * num_beams rows, cts_logprobs on those rows with k = keep (the per-row candidates: the
+ * union of every row's top `keep` holds the prompt's top `keep`), cts_beam_select, cts_beam_fork_kv.  Row b * num_beams + j is beam j
+ * of prompt b.
+ * cts_beam_select, one CTA per prompt.  Replaces, per step:
+ *   log_probs + running_beam_scores -> topk(beams_to_keep)        (_get_top_k_continuations; ties: the smaller beam * vocab + id)
+ *   stopping_criteria (EOS ids, max length)
+ *   _get_running_beams_for_next_iteration                           (ties: the better-ranked candidate)
+ *   _update_finished_beams                                           (score / len_den[step + 1]; ties: the older finished slot)
+ *   _check_early_stop_heuristic, _beam_search_has_unfinished_sequences (per prompt: prompt_flags[b] = {unsatisfied, done})
+ *   past_key_values.reorder_cache(beam_idx)                          (page-table rows + the fork descriptors below)
+ *   cand_ids / cand_logprobs [rows, keep]: per row the top `keep` (id, log-prob) of cts_logprobs; keep = max(2, 1 + n_eos) * num_beams.
+ *     The ids of one row must be distinct (as cts_logprobs gives them): the ranking assumes every (score, beam * vocab + id) is unique
+ *   len_den float [max_new + 1]: len_den[L] = (float)(L ** length_penalty), computed in double on the host as transformers does
+ *   early_stopping: 0 False, 1 True, 2 "never"
+ *   run_scores [rows]; fin_scores [rows] and fin_info int [rows, 4] = {step, parent row, token, finished}: the num_beams finished
+ *     slots of each prompt, best first (the hypothesis is the parent row's history at step - 1, then token)
+ *   step_ptr int[2] = {step, arrival counter}, zeroed before the first of at most max_new launches (a launch past max_new reads the
+ *     last len_den entry and writes no back-pointer); bp_tokens / bp_parents int [max_new, rows]: the token and parent row of every beam row
+ *     at every step; cur_ids / positions / seq_lens / slot_map advance as in cts_greedy_advance
+ *   page_table [rows, max_pages] is rewritten through page_table_old (same shape, scratch): pages below the tail column come from the
+ *     parent's row; the tail is own_pages[row, col] when the new position opens a page, else spare_pages[row] when the parent is
+ *     another row (the old tail becomes the spare, fork[row] = {parent's old tail, new tail, rows to copy}), else it stays.
+ *   A prompt whose done flag is set keeps its rows running and its finished slots unchanged.
+ * cts_beam_fork_kv: for every row with fork[row * 3 + 2] = n > 0, copies rows [0, n) of page fork[row * 3] into page fork[row * 3 + 1]
+ *   in every layer, K and V, of kv [layers, 2, num_pages, nkv, page_size, head_dim] (16-bit elements).  Sources are old tails and
+ *   destinations spares, so swaps and cycles of parents are safe in one launch. */
+int cts_beam_select(cts_ctx* ctx, int batch, int num_beams, int keep, long long vocab, const int* cand_ids, const float* cand_logprobs,
+                    const int* eos_ids, int n_eos, const float* len_den, int max_new, int early_stopping, float length_penalty,
+                    float* run_scores, float* fin_scores, int* fin_info, int* prompt_flags, int* step_ptr, int* bp_tokens, int* bp_parents,
+                    int* cur_ids, int* positions, int* seq_lens, int* slot_map, int* page_table, int* page_table_old,
+                    const int* own_pages, int* spare_pages, int max_pages, int page_size, int* fork, void* stream);
+int cts_beam_fork_kv(cts_ctx* ctx, void* kv, int layers, long long num_pages, int nkv, int page_size, int head_dim, const int* fork,
+                     int rows, void* stream);
+
 /* Debug / profiling aid (csrc/trace.cuh): instrumented kernels append {tag, %globaltimer} records to `buf` (unsigned long long
  * [2 + 2*capacity]: [0] cursor, [1] capacity, then the records) -- the overlapped timeline of a CUDA-graph replay that ncu, which
  * serialises kernels, cannot show (tools/trace_decode_step.py).  buf = NULL switches it off (the default). */

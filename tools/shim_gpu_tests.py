@@ -63,9 +63,10 @@ torch.cuda.is_current_stream_capturing = lambda: False
 from tests.cuda_on_cpu.shim import shim_context  # noqa: E402
 from tests.cuda_on_cpu.fp8 import attach as _attach_fp8  # noqa: E402
 from tests.cuda_on_cpu.structured import attach as _attach_structured  # noqa: E402
+from tests.cuda_on_cpu.beam import attach as _attach_beam  # noqa: E402
 import tests.gpu_util as gu  # noqa: E402
 
-_ctx = _attach_structured(_attach_fp8(shim_context()))  # + the FP8 and structured-output kernels (own shim libraries, same runtime)
+_ctx = _attach_beam(_attach_structured(_attach_fp8(shim_context())))  # + the FP8, structured-output and beam-search kernels (own shim libraries, same runtime)
 from tests.cabi_double import TorchDouble as _TD  # noqa: E402
 _dbl = _TD()
 # HYBRID context for the whole-step tests: every entry point whose source is in the shim build runs that source; the others (wgmma
@@ -146,6 +147,8 @@ SELECT = {
     "test_gpu_structured.py": "(mask_build and (1000 or 1003) and not 4096) or (mask_apply and not 152064) or struct_advance "
                               "or argument_errors",
     "test_gpu_zz_k_structured.py": "(choice and 4) or (regex and col) or (single_string and bfloat16) or logprobs_never",
+    # beam search: the selection kernel against its restatement and the copy-on-write fork of the KV pages, at the small shapes
+    "test_gpu_beam.py": "small",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
