@@ -35,6 +35,7 @@ SYMBOLS = [
     "cts_logprobs_workspace_floats", "cts_logprobs",
     "cts_struct_mask_build", "cts_struct_mask_apply", "cts_struct_advance",
     "cts_beam_select", "cts_beam_fork_kv",
+    "cts_logit_proc_apply", "cts_logit_proc_update",
 ]
 LOGPROBS_MAX_K = 20
 FUSED_RESIDUAL, FUSED_SWIGLU, FUSED_QKV_ROPE = 0, 1, 2
@@ -213,6 +214,10 @@ def load_library():
     lib.cts_beam_fork_kv.argtypes = [vp, vp, i, ll, i, i, i, vp, i, vp]
     for name in ("cts_beam_select", "cts_beam_fork_kv"):
         getattr(lib, name).restype = i
+    lib.cts_logit_proc_apply.argtypes = [vp, vp, ll, ll, i, vp, vp, vp, vp, i, vp, vp, i, vp, vp, vp, vp, i, i, vp]
+    lib.cts_logit_proc_update.argtypes = [vp, vp, i, ll, vp, i, vp, vp, vp]
+    for name in ("cts_logit_proc_apply", "cts_logit_proc_update"):
+        getattr(lib, name).restype = i
     # ---- A9: LoRA fine-tune step
     lib.cts_attn_prefill_lse.argtypes = [vp, vp, vp, vp, vp, i, i, ll, i, i, i, f, vp, vp, i, vp]
     lib.cts_attn_bwd.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i, i, ll, i, i, i, f, vp, vp, vp, vp, i, vp]
@@ -247,6 +252,16 @@ def dtype_code(dt):
     if dt == torch.float16:
         return F16
     raise CtsError(f"unsupported model dtype {dt}: the sm_90a kernels compute in bf16 or fp16 with fp32 accumulate")
+
+
+def _check_rows(fn, rows, specs):
+    """Each (tensor or None, dtype, ndim): the dtype, contiguous, at least ``rows`` rows -- the kernels index these tables by row."""
+    for t, dt, nd in specs:
+        if t is None:
+            continue
+        if t.dtype != dt or t.dim() != nd or not t.is_contiguous() or t.shape[0] < rows:
+            raise CtsError(f"{fn}: expected a contiguous {dt} tensor of {nd} dims and >= {rows} rows, got {t.dtype} {tuple(t.shape)}"
+                           f"{'' if t.is_contiguous() else ' (not contiguous)'}")
 
 
 def _p(t):
@@ -659,6 +674,34 @@ class Context:
         """Copy-on-write of the forked rows' partial tail pages in kv [L, 2, num_pages, nkv, page_size, d] (cts_beam_fork_kv)."""
         L, _, P, nkv, ps, d = kv.shape
         self._chk(self.lib.cts_beam_fork_kv(self.h, _p(kv), L, P, nkv, ps, d, _p(fork), int(rows), _stream()))
+
+    def logit_proc_apply(self, logits, batch, rep, presence, frequency, seen, counts, bias, bias_row, n_generated, min_tokens, stop_ids,
+                         vocab=None):
+        """Logits processors over rows x logits[:, :vocab] in place (cts_logit_proc_apply; shapes in include/chatts_b200.h).  counts
+        int16 [batch, vocab] read as uint16, or None; bias float32 [n_bias, vocab] or None; stop_ids int32 [batch, max_stop]."""
+        vocab = logits.shape[-1] if vocab is None else vocab
+        i32, f32 = torch.int32, torch.float32
+        _check_rows("logit_proc_apply", batch, [(rep, f32, 1), (presence, f32, 1), (frequency, f32, 1), (bias_row, i32, 1),
+                                                (n_generated, i32, 1), (min_tokens, i32, 1), (seen, i32, 2), (counts, torch.int16, 2),
+                                                (stop_ids, i32, 2)])
+        _check_rows("logit_proc_apply", 0, [(bias, f32, 2)])
+        for name, t in (("counts", counts), ("bias", bias)):
+            if t is not None and t.shape[1] != vocab:
+                raise CtsError(f"logit_proc_apply: {name} rows must hold exactly vocab = {vocab} entries, got {t.shape[1]}")
+        ms = stop_ids.shape[1] if stop_ids is not None else 0
+        self._chk(self.lib.cts_logit_proc_apply(self.h, _p(logits), int(vocab), logits.stride(0), int(batch), _p(rep), _p(presence),
+                                                _p(frequency), _p(seen), seen.shape[1], _p(counts), _p(bias),
+                                                bias.shape[0] if bias is not None else 0, _p(bias_row), _p(n_generated), _p(min_tokens),
+                                                _p(stop_ids) if ms else None, ms, dtype_code(logits.dtype), _stream()))
+
+    def logit_proc_update(self, cur_ids, batch, seen, counts, n_generated, vocab):
+        """After an advance: counts[b, cur_ids[b]] += 1, the seen bit set, n_generated[b] += 1 (cts_logit_proc_update)."""
+        _check_rows("logit_proc_update", batch, [(cur_ids, torch.int32, 1), (n_generated, torch.int32, 1), (seen, torch.int32, 2),
+                                                 (counts, torch.int16, 2)])
+        if counts is not None and counts.shape[1] != vocab:
+            raise CtsError(f"logit_proc_update: counts rows must hold exactly vocab = {vocab} entries, got {counts.shape[1]}")
+        self._chk(self.lib.cts_logit_proc_update(self.h, _p(cur_ids), int(batch), int(vocab), _p(seen), seen.shape[1], _p(counts),
+                                                 _p(n_generated), _stream()))
 
     # ------------------------------------------------------------------ A9: LoRA fine-tune step
     def attn_prefill_lse(self, q, k, v, cu_seqlens, batch, max_seqlen, nh, nkv, head_dim, scale, out, lse):

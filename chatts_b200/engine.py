@@ -13,7 +13,9 @@ between two replays by rewriting its slot's few integers:
     always runs at its full width, the price of never re-capturing.
 
 Greedy decoding; per-row arithmetic does not depend on the other rows, so a request produces the tokens a stand-alone
-``generate()`` call produces.  Host logic only (torch copies of a few int32 per slot); every number comes from the kernels.
+``generate()`` call produces.  A request may carry vLLM's logits processors (chatts_b200.logit_proc), one parameter set per slot: a
+round in which some active slot uses them runs each step as the decode step without its advance, cts_logit_proc_apply over every slot
+(neutral and free slots are skipped), the greedy advance and cts_logit_proc_update; a round in which none does replays the plain graph.  Host logic only (torch copies of a few int32 per slot); every number comes from the kernels.
 """
 from collections import deque
 from dataclasses import dataclass, field
@@ -21,6 +23,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
+from . import logit_proc as lpmodp
 from . import logprobs as lpmod
 from ._cabi import LOGPROBS_MAX_K
 
@@ -41,6 +44,7 @@ class Request:
     cached_positions: int = 0          # prompt positions whose KV came from the prefix cache (model built with enable_prefix_caching)
     logprobs: int = None               # top-k of the logprobs asked for (None: none)
     token_logprobs: list = field(default_factory=list)   # per token: (logprob, rank, top-k ids, top-k logprobs), as in generate()
+    procs: lpmodp.Processors = None    # logits processors (None: none)
 
 
 class ContinuousEngine:
@@ -66,17 +70,25 @@ class ContinuousEngine:
         self.rounds = 0
         self.occupancy = []                                # active slots per round (observability / tests)
         self._lpb = None                                   # logprob outputs of a round, made when a request first asks
+        self._proc = None                                  # per-slot logits processors, made when a request first asks
 
     # ------------------------------------------------------------------------------------------ public
-    def add_request(self, input_ids, series=None, max_new_tokens=16, eos_token_id=None, ignore_eos=False, logprobs=None):
-        """logprobs = k (0..20): every token's logprob and rank and the k most likely tokens, in Request.token_logprobs."""
+    def add_request(self, input_ids, series=None, max_new_tokens=16, eos_token_id=None, ignore_eos=False, logprobs=None,
+                    presence_penalty=0.0, frequency_penalty=0.0, repetition_penalty=None, logit_bias=None, allowed_token_ids=None,
+                    min_tokens=None):
+        """logprobs = k (0..20): every token's logprob and rank and the k most likely tokens, in Request.token_logprobs.
+        presence_penalty, frequency_penalty, repetition_penalty, logit_bias, allowed_token_ids, min_tokens: the logits processors of
+        generate() (its min_new_tokens is min_tokens here), from the first token on; ValueError on a bad value."""
         k = lpmod.check_k(logprobs, "logprobs")
         cfg = self.m.config
+        procs = lpmodp.resolve(presence_penalty, frequency_penalty, repetition_penalty, logit_bias, allowed_token_ids, min_tokens,
+                               max_new_tokens, vocab=cfg.vocab_size)
         eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
         eos = set(eos) if isinstance(eos, (list, tuple, set)) else {int(eos)}
+        lpmodp.check_stop_ids(procs, [] if ignore_eos else eos)
         ids = torch.as_tensor(input_ids, dtype=torch.long).reshape(-1)
         ts = series if series is not None else torch.zeros(0, 0, 1)
-        r = Request(self._next, ids, ts, int(max_new_tokens), eos, ignore_eos, logprobs=k)
+        r = Request(self._next, ids, ts, int(max_new_tokens), eos, ignore_eos, logprobs=k, procs=procs)
         self._next += 1
         self.waiting.append(r)
         return r.rid
@@ -177,7 +189,18 @@ class ContinuousEngine:
             t_pos, t_seq = lens32 - 1, lens32.clone()
             t_slot = torch.zeros(g, dtype=torch.int32, device=dev)
             t_pt = torch.from_numpy(pts).to(dev)
+            pslots = [free[i] for i, r in enumerate(group) if r.procs is not None]
+            if pslots:                                     # the group's processors, on the first token's (prefill) logits
+                self._set_procs([r for r in group if r.procs is not None], pslots)
+                rows = [i for i, r in enumerate(group) if r.procs is not None]
+                sub = logits[rows]
+                self._proc.apply_rows(sub, pslots)
+                logits[rows] = sub
             m.ctx.greedy_advance(logits, g, t_out, t_step, t_cur, t_pos, t_seq, t_slot, t_pt, m.page_size)
+            if pslots:
+                cur = torch.full((self.B,), -1, dtype=torch.int32, device=dev)      # -1: rows the update leaves alone
+                cur[torch.tensor(pslots, device=dev)] = t_cur[torch.tensor(rows, device=dev)]
+                self._proc.update(cur, self.B)
             ks = [r.logprobs for r in group if r.logprobs is not None]
             if ks:                                         # the first token's logprobs, from the prefill logits
                 lpb = lpmod.LogprobBuffers(m.ctx, g, 1, max(ks), m.config.vocab_size, dev)
@@ -215,6 +238,16 @@ class ContinuousEngine:
         finally:
             self.waiting.extend(rest)
 
+    def _set_procs(self, reqs, slots):
+        m = self.m
+        if self._proc is None:
+            self._proc = lpmodp.LogitProcState(m.ctx, self.B, m.config.vocab_size, m.n_pos, m.device)
+        for r, slot in zip(reqs, slots):
+            self._proc.set_rows([slot], r.procs, [] if r.ignore_eos else r.eos, shared_bias=False)
+            if r.procs.repetition_penalty != 1:            # the prompt ids, as generate() marks them
+                tok = r.input_ids.to(torch.int32).to(m.device)
+                self._proc.mark_prompt(tok, torch.full_like(tok, slot))
+
     def _fail(self, r, err):
         r.error, r.done = err, True
         self.finished.append(r)
@@ -229,8 +262,16 @@ class ContinuousEngine:
         ks = [r.logprobs for r in self.active.values() if r.logprobs is not None]
         if ks and self._lpb is None:
             self._lpb = lpmod.LogprobBuffers(m.ctx, self.B, self.k, LOGPROBS_MAX_K, m.config.vocab_size, m.device)
+        procs = any(r.procs is not None for r in self.active.values())
         for _ in range(self.k):
-            m._decode_step(st, sample=True)
+            if procs:
+                m._decode_step(st, sample=False)
+                self._proc.apply(st.full_logits, self.B)
+                m.ctx.greedy_advance(st.full_logits, self.B, st.out_tokens, st.step_ptr, st.cur_ids, st.positions, st.seq_lens, st.slot_map,
+                                     st.page_table, m.page_size)
+                self._proc.update(st.cur_ids, self.B)
+            else:
+                m._decode_step(st, sample=True)
             if ks:                                         # all slots at the largest k asked; columns from step_ptr
                 self._lpb.launch(st.full_logits, self.B, st.out_tokens, k=max(ks), step_ptr=st.step_ptr)
         toks = st.out_tokens[:, : self.k].cpu().numpy()    # the round's one device->host read
@@ -270,6 +311,8 @@ class ContinuousEngine:
             self.m.pool.release(r.pages)
             r.pages = []
         if r.slot >= 0:
+            if r.procs is not None:
+                self._proc.reset_rows([r.slot])
             self.st.page_table[r.slot].fill_(self.scratch)
             self._reset_free([r.slot])
 

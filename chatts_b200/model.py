@@ -19,6 +19,7 @@ import torch
 
 from . import _cabi, layout, prefix_cache, structured
 from . import beam as beammod
+from . import logit_proc as lpmodp
 from . import logprobs as lpmod
 from .trace import span
 from ._cabi import EPI_NONE, EPI_PARTIAL_F32, EPI_RESIDUAL, EPI_SWIGLU_IL
@@ -1102,7 +1103,8 @@ class ChatTSForCausalLM:
                  do_sample=None, temperature=None, top_p=None, top_k=None, streamer=None, eos_token_id=None, pad_token_id=None,
                  synced_gpus=False, sync_every=16, ignore_eos=False, seed=None, repetition_penalty=None, logprobs=None,
                  prompt_logprobs=None, structured_outputs=None, tokenizer=None, num_beams=None, length_penalty=1.0, early_stopping=False,
-                 num_return_sequences=1, num_beam_groups=None, diversity_penalty=None, **_):
+                 num_return_sequences=1, num_beam_groups=None, diversity_penalty=None, presence_penalty=0.0, frequency_penalty=0.0,
+                 logit_bias=None, allowed_token_ids=None, min_new_tokens=None, **_):
         """model.generate(**processor_out, max_new_tokens=...) -> LongTensor [B, S + new] whose first S columns are
         the ORIGINAL (un-expanded) input ids (README.md:102-103).
 
@@ -1124,7 +1126,14 @@ class ChatTSForCausalLM:
         "never") and ``num_return_sequences`` (<= num_beams) as there.  Returns [B * num_return_sequences, S + n], each prompt's best
         hypotheses first, padded with pad_token_id; ``self.last_beam_scores`` holds their scores (transformers' sequences_scores, fp32),
         and is None after any other call.  Greedy only (do_sample, repetition_penalty != 1, logprobs, structured outputs, a streamer
-        and tensor parallelism are refused with ValueError), and max(2, 1 + number of EOS ids) * num_beams <= 20."""
+        and tensor parallelism are refused with ValueError), and max(2, 1 + number of EOS ids) * num_beams <= 20.
+
+        presence_penalty, frequency_penalty (each in [-2, 2]), logit_bias ({token id: bias}, clamped to [-100, 100]), allowed_token_ids
+        and min_new_tokens (vLLM's min_tokens: the stop ids are refused until a row has generated that many tokens): vLLM's logits
+        processors, applied every step by cts_logit_proc_apply (chatts_b200.logit_proc states the order), together with
+        repetition_penalty, after the structured-output mask and before temperature, top-k and top-p; the logprobs describe the
+        processed logits.  Not with beam search or tensor parallelism; allowed_token_ids and min_new_tokens not with
+        structured_outputs."""
         cfg, dev = self.config, self.device
         lpk, plk = lpmod.check_k(logprobs, "logprobs"), lpmod.check_k(prompt_logprobs, "prompt_logprobs")
         if (lpk is not None or plk is not None) and self.tp_size > 1:
@@ -1134,6 +1143,17 @@ class ChatTSForCausalLM:
             raise ValueError("structured_outputs are single-GPU only (tensor_parallel_size must be 1)")
         if so is not None and ignore_eos:
             raise ValueError("structured_outputs end the output with a stop id: they cannot be combined with ignore_eos")
+        procs = lpmodp.resolve(presence_penalty, frequency_penalty, None, logit_bias, allowed_token_ids, min_new_tokens,
+                               vocab=cfg.vocab_size)
+        if procs is not None:
+            if num_beams not in (None, 1):
+                raise ValueError("presence_penalty, frequency_penalty, logit_bias, allowed_token_ids and min_new_tokens do not work with "
+                                 "beam search (num_beams > 1)")
+            if self.tp_size > 1:
+                raise ValueError("logits processors are single-GPU only (tensor_parallel_size must be 1)")
+            if so is not None and (procs.allowed_token_ids is not None or procs.min_tokens > 0):
+                raise ValueError("allowed_token_ids and min_new_tokens cannot be combined with structured_outputs: either can refuse "
+                                 "every token the automaton allows")
         self.last_logprobs = None
         gd = getattr(self, "generation_defaults", None)
         if gd:                                          # checkpoint defaults apply only where the caller said nothing
@@ -1172,6 +1192,14 @@ class ChatTSForCausalLM:
             return torch.as_tensor(ids_cpu, dtype=torch.long)
         eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
         eos_set = set(eos) if isinstance(eos, (list, tuple, set)) else {int(eos)}
+        if procs is not None:
+            if procs.min_tokens > max_new_tokens:
+                raise ValueError(f"min_new_tokens ({procs.min_tokens}) must be <= max_new_tokens ({max_new_tokens})")
+            lpmodp.check_stop_ids(procs, [] if ignore_eos else eos_set)
+            rp = repetition_penalty if repetition_penalty is not None else 1.0
+            if not rp > 0:
+                raise ValueError(f"repetition_penalty must be > 0, got {repetition_penalty}")
+            procs.repetition_penalty = float(rp)
         pad = cfg.pad_token_id if pad_token_id is None else pad_token_id
         auto = None
         if so is not None:
@@ -1230,7 +1258,17 @@ class ChatTSForCausalLM:
             # logits are rewritten by cts_rep_penalty_apply before the argmax / sampling kernel, the new token is marked after it
             rep = float(repetition_penalty) if repetition_penalty not in (None, 1, 1.0) else None
             seen = None
-            if rep is not None:
+            proc = None
+            if procs is not None:
+                # every other processor on: cts_logit_proc_apply takes over the repetition penalty, its update marks the new tokens
+                proc = lpmodp.LogitProcState(self.ctx, B, self.config.vocab_size, self.n_pos, dev)
+                proc.set_rows(list(range(B)), procs, [] if ignore_eos else eos_set, shared_bias=True)
+                if rep is not None:
+                    am = np.ones_like(ids_cpu) if am_cpu is None else am_cpu
+                    rr, cc = np.nonzero(am)
+                    proc.mark_prompt(torch.from_numpy(ids_cpu[rr, cc].astype(np.int32)).to(dev), torch.from_numpy(rr.astype(np.int32)).to(dev))
+                proc.apply(logits, B)
+            elif rep is not None:
                 Vfull = self.config.vocab_size
                 seen = torch.zeros(B, (Vfull + 31) // 32, dtype=torch.int32, device=dev)
                 am = np.ones_like(ids_cpu) if am_cpu is None else am_cpu
@@ -1245,7 +1283,9 @@ class ChatTSForCausalLM:
                                             st.page_table, self.page_size)
                 else:
                     sample(lg, step)
-                if seen is not None:
+                if proc is not None:
+                    proc.update(st.cur_ids, B)
+                elif seen is not None:
                     self.ctx.rep_penalty_mark(st.cur_ids, None, seen, self.config.vocab_size)
                 if auto is not None:
                     auto.advance(self.ctx, st.cur_ids, B, struct_state)
@@ -1284,13 +1324,15 @@ class ChatTSForCausalLM:
                     if produced >= max_new_tokens or done.all():
                         break
                 with span("cts.decode_step"):
-                    if greedy and seen is None and auto is None:
+                    if greedy and seen is None and auto is None and proc is None:
                         self._decode_step(st, sample=True)
                     else:
                         self._decode_step(st, sample=False)
                         if auto is not None:
                             auto.mask_apply(self.ctx, st.full_logits, B, struct_state)
-                        if seen is not None:
+                        if proc is not None:
+                            proc.apply(st.full_logits, B)
+                        elif seen is not None:
                             self.ctx.rep_penalty_apply(st.full_logits, B, seen, rep)
                         advance(st.full_logits, produced)
                     if lpb is not None:

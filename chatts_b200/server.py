@@ -22,6 +22,7 @@ import uuid
 from concurrent.futures import Future
 from dataclasses import dataclass, field
 
+from .logit_proc import resolve as resolve_processors
 from .logprobs import check_k
 from .structured import compile_params, resolve as resolve_structured
 from .vllm_compat import IncrementalDecoder, decode_text, eos_ids
@@ -152,8 +153,7 @@ class Engine:
         """Iteration-level batching (engine.ContinuousEngine): requests join the static decode slots between graph replays and
         leave them at EOS / max_tokens; streaming requests get their new tokens after every round."""
         from .engine import ContinuousEngine
-        from .vllm_compat import (CompletionOutput, RequestOutput, cut_at_stop, cut_at_stop_string, decode_text, logprob_dict,
-                                  tokens_before_stop_string)
+        from .vllm_compat import CompletionOutput, RequestOutput, cut_at_stop, cut_at_stop_string_after, logprob_dict, tokens_before_stop_string
         llm = self.llm
         eng = ContinuousEngine(llm.model, steps_per_round=self.steps_per_round)
         jobs, sent = {}, {}
@@ -165,7 +165,8 @@ class Engine:
                 gd = getattr(llm.model, "generation_defaults", None) or {}
                 job.stop_ids = eos_ids(llm.model.config, p.get("stop_token_ids"), gd.get("eos_token_id"))
                 rid = eng.add_request(enc["input_ids"][0], enc["timeseries"], max_new_tokens=p.get("max_tokens", 16),
-                                      eos_token_id=job.stop_ids, ignore_eos=p.get("ignore_eos", False), logprobs=p.get("logprobs"))
+                                      eos_token_id=job.stop_ids, ignore_eos=p.get("ignore_eos", False), logprobs=p.get("logprobs"),
+                                      **{k: p[k] for k in PROCESSOR_FIELDS if k in p})
                 jobs[rid], sent[rid] = job, 0
                 if job.stream_q is not None:
                     job.decoder = IncrementalDecoder(llm.tokenizer)
@@ -176,11 +177,11 @@ class Engine:
 
         def finish(job, r):
             toks, fin = cut_at_stop(r.tokens, job.stop_ids, job.params.get("ignore_eos", False))
-            stops = job.params.get("stop") or []
-            text, hit = cut_at_stop_string(decode_text(llm.tokenizer, toks), stops)
+            stops, mt = job.params.get("stop") or [], job.params.get("min_tokens", 0)
+            text, hit = cut_at_stop_string_after(llm.tokenizer, toks, stops, mt)
             out = CompletionOutput(text, toks, "stop" if hit else fin)
             if r.logprobs is not None:
-                keep = tokens_before_stop_string(llm.tokenizer, toks, stops) if hit else len(toks)
+                keep = tokens_before_stop_string(llm.tokenizer, toks, stops, mt) if hit else len(toks)
                 out.logprobs = [logprob_dict(toks[j], *r.token_logprobs[j], llm.tokenizer) for j in range(keep)]
                 out.cumulative_logprob = float(sum(r.token_logprobs[j][0] for j in range(keep)))
             return out
@@ -280,10 +281,15 @@ def _structured_from_body(body):
     return {"choice": list(so.choice)} if so.choice is not None else {"regex": so.regex}
 
 
+PROCESSOR_FIELDS = ("presence_penalty", "frequency_penalty", "repetition_penalty", "logit_bias", "allowed_token_ids", "min_tokens")
+
+
 def _sampling_from_body(body, chat=False):
     """SamplingParams fields of an OpenAI request body.  Log probabilities: chat takes ``logprobs: true`` with ``top_logprobs`` 0..20,
     completions ``logprobs: <int>`` 0..20; neither works with ``stream`` (ValueError, a 400 for the client).  Constraints:
-    ``structured_outputs`` ({"choice": [...]} or {"regex": "..."}) or ``guided_choice`` / ``guided_regex``."""
+    ``structured_outputs`` ({"choice": [...]} or {"regex": "..."}) or ``guided_choice`` / ``guided_regex``.  Logits processors:
+    ``presence_penalty``, ``frequency_penalty``, ``logit_bias``, ``repetition_penalty``, ``min_tokens``, ``allowed_token_ids``, each
+    kept only when present and not neutral (so requests without them still batch together)."""
     p = {"max_tokens": int(body.get("max_tokens") or body.get("max_completion_tokens") or 256),
          "temperature": float(body.get("temperature", 0.0) or 0.0), "top_p": float(body.get("top_p", 1.0) or 1.0),
          "top_k": int(body.get("top_k", 0) or 0), "n": int(body.get("n", 1) or 1)}
@@ -315,6 +321,21 @@ def _sampling_from_body(body, chat=False):
         if p.get("ignore_eos"):
             raise ValueError("structured_outputs end the output with a stop id: they cannot be combined with ignore_eos")
         p["structured_outputs"] = so
+    procs = resolve_processors(body.get("presence_penalty"), body.get("frequency_penalty"), body.get("repetition_penalty"),
+                               body.get("logit_bias"), body.get("allowed_token_ids"), body.get("min_tokens"), p["max_tokens"])
+    if procs is not None:
+        if procs.presence_penalty != 0:
+            p["presence_penalty"] = procs.presence_penalty
+        if procs.frequency_penalty != 0:
+            p["frequency_penalty"] = procs.frequency_penalty
+        if procs.repetition_penalty != 1:
+            p["repetition_penalty"] = procs.repetition_penalty
+        if procs.logit_bias is not None:
+            p["logit_bias"] = procs.logit_bias
+        if procs.allowed_token_ids is not None:
+            p["allowed_token_ids"] = procs.allowed_token_ids
+        if procs.min_tokens > 0:
+            p["min_tokens"] = procs.min_tokens
     return p
 
 

@@ -9,6 +9,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
+from . import logit_proc as lpmodp
 from . import logprobs as lpmod
 from .config import ChatTSConfig
 from .model import ChatTSForCausalLM
@@ -35,8 +36,17 @@ class SamplingParams:
     logprobs: int = None                              # 0..20: logprob of every generated token plus its top-k (single GPU)
     prompt_logprobs: int = None                       # 0..20: the same for every prompt token after the first (single GPU)
     structured_outputs: StructuredOutputsParams = None  # choice / regex constraint on the output (a dict of its fields is accepted)
+    presence_penalty: float = 0.0                     # [-2, 2]: subtracted once from every token the output already holds
+    frequency_penalty: float = 0.0                    # [-2, 2]: subtracted per occurrence in the output
+    logit_bias: dict = None                           # {token id (int or str): bias}, clamped to [-100, 100]
+    allowed_token_ids: list = None                    # only these ids may be generated
+    min_tokens: int = 0                               # stop ids and stop strings do not end the output before this many tokens
 
     def __post_init__(self):
+        procs = lpmodp.resolve(self.presence_penalty, self.frequency_penalty, self.repetition_penalty, self.logit_bias,
+                               self.allowed_token_ids, self.min_tokens, self.max_tokens)
+        if procs is not None:
+            self.logit_bias = procs.logit_bias
         lpmod.check_k(self.logprobs, "logprobs")
         lpmod.check_k(self.prompt_logprobs, "prompt_logprobs")
         self.structured_outputs = _resolve_structured(self.structured_outputs)
@@ -83,15 +93,25 @@ def prompt_logprob_dicts(entries, tokenizer):
     return [None if e is None else logprob_dict(e.token_id, e.logprob, e.rank, e.top_ids, e.top_logprobs, tokenizer) for e in entries]
 
 
-def tokens_before_stop_string(tokenizer, tokens, stops):
+def tokens_before_stop_string(tokenizer, tokens, stops, min_tokens=0):
     """The number of leading tokens whose text first contains a stop string (all of them when none does): the tokens the cut text
-    came from, the one that completed the stop string included."""
+    came from, the one that completed the stop string included.  min_tokens as in cut_at_stop_string_after."""
     if not any(stops):
         return len(tokens)
     for n in range(1, len(tokens) + 1):
-        if cut_at_stop_string(decode_text(tokenizer, tokens[:n]), stops)[1]:
+        if cut_at_stop_string_after(tokenizer, tokens[:n], stops, min_tokens)[1]:
             return n
     return len(tokens)
+
+
+def cut_at_stop_string_after(tokenizer, tokens, stops, min_tokens=0):
+    """cut_at_stop_string of the decoded tokens: the text before the earliest-starting stop string.  With min_tokens > 0 only an
+    occurrence that ends after the text of the first min_tokens tokens counts: vLLM's stop checker looks for stop strings in the new
+    text of a step only once the output is longer than min_tokens, so one that completes earlier never ends the output."""
+    text = decode_text(tokenizer, tokens)
+    floor = len(decode_text(tokenizer, tokens[:min_tokens])) if min_tokens else 0
+    starts = [i for st in stops if st for i in [text.find(st, max(0, floor - len(st) + 1))] if i >= 0]
+    return (text[:min(starts)], True) if starts else (text, False)
 
 
 def eos_ids(config, stop_token_ids=None, extra=None):
@@ -340,16 +360,18 @@ class LLM:
                                       eos_token_id=stop_ids, streamer=streamer,
                                       repetition_penalty=(sp.repetition_penalty if sp.repetition_penalty not in (None, 1.0) else None),
                                       logprobs=sp.logprobs, prompt_logprobs=sp.prompt_logprobs,
-                                      structured_outputs=sp.structured_outputs, tokenizer=self.tokenizer)
+                                      structured_outputs=sp.structured_outputs, tokenizer=self.tokenizer,
+                                      presence_penalty=sp.presence_penalty, frequency_penalty=sp.frequency_penalty, logit_bias=sp.logit_bias,
+                                      allowed_token_ids=sp.allowed_token_ids, min_new_tokens=sp.min_tokens)
             res = self.model.last_logprobs if (sp.logprobs is not None or sp.prompt_logprobs is not None) else None
             for b, req in enumerate(chunk):
                 # a row ends at ITS first stop id (the batch-wide tail after it is the pad fill of generate())
                 toks, fin = cut_at_stop(ids[b, S:].tolist(), stop_ids, sp.ignore_eos)
-                text, hit = cut_at_stop_string(decode_text(self.tokenizer, toks), stops)
+                text, hit = cut_at_stop_string_after(self.tokenizer, toks, stops, sp.min_tokens)
                 hits = getattr(self.model, "last_cached_positions", None)
                 co = CompletionOutput(text, toks, "stop" if hit else fin)
                 if sp.logprobs is not None:
-                    keep = tokens_before_stop_string(self.tokenizer, toks, stops) if hit else len(toks)
+                    keep = tokens_before_stop_string(self.tokenizer, toks, stops, sp.min_tokens) if hit else len(toks)
                     co.logprobs, co.cumulative_logprob = completion_logprobs(res, b, keep, toks, self.tokenizer)
                 plp = prompt_logprob_dicts(res.prompt[b], self.tokenizer) if sp.prompt_logprobs is not None else None
                 outs.append(RequestOutput(req["prompt"], [co], int(hits[b]) if hits is not None else 0, plp))
@@ -440,7 +462,7 @@ class AsyncLLMEngine:
                 continue
             toks += item
             text = decode_text(self.llm.tokenizer, toks)
-            if any(st and st in text for st in stops):
+            if cut_at_stop_string_after(self.llm.tokenizer, toks, stops, sp.min_tokens)[1]:
                 continue                               # the final output carries the text cut at the stop string
             if text.endswith("\ufffd"):
                 continue                               # incomplete multi-byte character: wait for the bytes that complete it

@@ -649,6 +649,28 @@ int cts_beam_select(cts_ctx* ctx, int batch, int num_beams, int keep, long long 
 int cts_beam_fork_kv(cts_ctx* ctx, void* kv, int layers, long long num_pages, int nkv, int page_size, int head_dim, const int* fork,
                      int rows, void* stream);
 
+/* Logits processors (csrc/logit_proc.cu; chatts_b200/logit_proc.py): vLLM's allowed_token_ids, logit_bias, min_tokens and its
+ * repetition / presence / frequency penalties in one pass over 16-bit logits [batch, ld], run after the structured-output mask and
+ * before the greedy / sample advance.  Every parameter is per row, on the device:
+ *   rep, presence, frequency  float [batch]   (1, 0, 0: neutral)
+ *   seen        uint32 [batch, words_per_row]: the occurrence bits of cts_rep_penalty_mark (prompt and generated ids)
+ *   counts      uint16 [batch, vocab]: occurrences of each id among the row's GENERATED tokens (NULL: presence / frequency off)
+ *   bias        float [n_bias, vocab], bias_row int [batch] (-1 or >= n_bias: none): added to the logits; -inf marks an id outside
+ *               allowed_token_ids, whose logit becomes -inf
+ *   n_generated, min_tokens int [batch]; stop_ids int [batch, max_stop] (max_stop <= 64, padded with -1): while n_generated < min_tokens
+ *               the row's stop ids get -inf
+ * cts_logit_proc_apply: per entry, in fp32 and rounded once: allowed mask, + bias, min_tokens, repetition penalty (as
+ *   cts_rep_penalty_apply), then x = (x - frequency * c) - presence where c = counts > 0.  An entry no step changes keeps its bits; a
+ *   row with neutral parameters is not written.  With only rep set the result is bit-identical to cts_rep_penalty_apply.
+ * cts_logit_proc_update: after the advance, per row with 0 <= cur_ids[b] < vocab: counts[b, id] += 1 (counts may be NULL), the seen
+ *   bit set, n_generated[b] += 1; rows with an id outside [0, vocab) are left unchanged. */
+int cts_logit_proc_apply(cts_ctx* ctx, void* logits, long long vocab, long long ld, int batch, const float* rep, const float* presence,
+                         const float* frequency, const unsigned* seen, int words_per_row, const unsigned short* counts, const float* bias,
+                         int n_bias, const int* bias_row, const int* n_generated, const int* min_tokens, const int* stop_ids, int max_stop,
+                         int dtype, void* stream);
+int cts_logit_proc_update(cts_ctx* ctx, const int* cur_ids, int batch, long long vocab, unsigned* seen, int words_per_row,
+                          unsigned short* counts, int* n_generated, void* stream);
+
 /* Debug / profiling aid (csrc/trace.cuh): instrumented kernels append {tag, %globaltimer} records to `buf` (unsigned long long
  * [2 + 2*capacity]: [0] cursor, [1] capacity, then the records) -- the overlapped timeline of a CUDA-graph replay that ncu, which
  * serialises kernels, cannot show (tools/trace_decode_step.py).  buf = NULL switches it off (the default). */

@@ -64,9 +64,11 @@ from tests.cuda_on_cpu.shim import shim_context  # noqa: E402
 from tests.cuda_on_cpu.fp8 import attach as _attach_fp8  # noqa: E402
 from tests.cuda_on_cpu.structured import attach as _attach_structured  # noqa: E402
 from tests.cuda_on_cpu.beam import attach as _attach_beam  # noqa: E402
+from tests.cuda_on_cpu.logit_proc import attach as _attach_logit_proc  # noqa: E402
 import tests.gpu_util as gu  # noqa: E402
 
-_ctx = _attach_beam(_attach_structured(_attach_fp8(shim_context())))  # + the FP8, structured-output and beam-search kernels (own shim libraries, same runtime)
+_ctx = _attach_logit_proc(_attach_beam(_attach_structured(_attach_fp8(shim_context()))))  # + the FP8, structured-output, beam-search and
+# logits-processor kernels (own shim libraries, same runtime)
 from tests.cabi_double import TorchDouble as _TD  # noqa: E402
 _dbl = _TD()
 # HYBRID context for the whole-step tests: every entry point whose source is in the shim build runs that source; the others (wgmma
@@ -149,6 +151,11 @@ SELECT = {
     "test_gpu_zz_k_structured.py": "(choice and 4) or (regex and col) or (single_string and bfloat16) or logprobs_never",
     # beam search: the selection kernel against its restatement and the copy-on-write fork of the KV pages, at the small shapes
     "test_gpu_beam.py": "small",
+    # logits processors: both kernels at the small vocabularies, and generate() / the engine on the tiny model
+    "test_gpu_logit_proc.py": "(apply_matches and not 152064 and not -32-) or row_stride or (rep_only and not 152064) "
+                              "or (update and not 152064) or argument_errors",
+    "test_gpu_zz_m_logit_proc.py": "(neutral and dt0) or (eos_bias and (None-4 or 7-4)) or (allowed and (None-4 or 3-4)) "
+                                   "or logprobs_describe or (continuous and dt0) or slot_reuse",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
