@@ -11,6 +11,11 @@
 //   top-p : the largest tau (>= tau_k) with  sum_{z_i >= tau} p_i >= top_p * mass(top-k set)     (ties at tau are all kept)
 // then one inverse-CDF pass in INDEX order over the kept set with a counter-based uniform u(seed, step, sequence)
 // (splitmix64), so a (seed, step) pair always gives the same token -- restated on the CPU in tests/cabi_double.py.
+// Each thread owns a contiguous chunk with an fp32 sum; the prefix over chunks and the target u * total are fp64, so a tail token
+// behind a dominant one (below ulp(1) of an fp32 prefix) keeps its share.  One block max names the single chunk that holds the
+// target, and that chunk is walked from 0 against the target's offset into it.  Only tokens with mass are ever returned: a -inf
+// logit (a structured-output or allowed-id refusal, a min_tokens stop id) never is.  A row without usable mass (no finite logit)
+// gives cts_greedy_advance's token.
 #include "common.cuh"
 
 namespace {
@@ -61,7 +66,8 @@ sample_advance_kernel(const T* __restrict__ logits, long long vocab, float inv_t
   pdl_trigger();
   pdl_wait();
   __shared__ float red[32];
-  __shared__ float scan_s[32];
+  __shared__ double scan_s[32];
+  __shared__ double total_s;
   __shared__ int winner_s;
   const int b = blockIdx.x;
   const T* row = logits + (long long)b * vocab;
@@ -125,14 +131,17 @@ sample_advance_kernel(const T* __restrict__ logits, long long vocab, float inv_t
   // ---- inverse CDF in index order over the kept set
   const int step = step_ptr ? step_ptr[0] : 0;
   const unsigned long long h = splitmix64(seed ^ splitmix64(((unsigned long long)(unsigned)step << 32) | (unsigned)b));
-  const float u = (float)(h >> 40) * (1.0f / 16777216.0f);                   // 24 random bits -> [0, 1)
+  const double u = (double)(h >> 40) * (1.0 / 16777216.0);                  // 24 random bits -> [0, 1)
   float loc = 0.f;
   visit([&](long long, float x, unsigned short bb) { if (x == x && key16(bb) >= tau) loc += prob(x); });
-  // block exclusive scan of the per-thread sums (threads own increasing index ranges)
-  float incl = loc;
+  // block exclusive scan of the per-thread sums (threads own increasing index ranges), in fp64: in fp32 a prefix near the total
+  // only resolves ulp(1) ~ 1.2e-7, more than a tail token behind a dominant one holds, and its rounding would both leave gaps
+  // between neighbouring chunks and line every chunk start up with the grid of fp32 targets (over-weighting each chunk's first
+  // token)
+  double incl = loc;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
-    const float n = __shfl_up_sync(0xffffffffu, incl, o);
+    const double n = __shfl_up_sync(0xffffffffu, incl, o);
     if ((threadIdx.x & 31) >= o) incl += n;
   }
   if (threadIdx.x == 0) winner_s = -1;
@@ -140,39 +149,42 @@ sample_advance_kernel(const T* __restrict__ logits, long long vocab, float inv_t
   if ((threadIdx.x & 31) == 31) scan_s[threadIdx.x >> 5] = incl;
   __syncthreads();
   if (threadIdx.x < 32) {
-    float w = scan_s[threadIdx.x], wi = w;
+    double w = scan_s[threadIdx.x], wi = w;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-      const float n = __shfl_up_sync(0xffffffffu, wi, o);
+      const double n = __shfl_up_sync(0xffffffffu, wi, o);
       if (threadIdx.x >= o) wi += n;
     }
     scan_s[threadIdx.x] = wi - w;                                            // exclusive prefix of the warp totals
-    if (threadIdx.x == 31) red[0] = wi;                                      // grand total (same summation tree every launch)
+    if (threadIdx.x == 31) total_s = wi;                                     // grand total (same summation tree every launch)
   }
   __syncthreads();
-  const float total = red[0];
-  const float excl = scan_s[threadIdx.x >> 5] + incl - loc;
-  float target = u * total;
-  if (target >= total) target = total * 0.99999994f;
-  if (loc > 0.f && target >= excl && target < excl + loc) {
-    float acc = excl;
-    int pick = -1;
-    long long last = -1;
+  const double rel = u * total_s - (scan_s[threadIdx.x >> 5] + (incl - loc));   // where the draw lies from this chunk's start
+  // the owner of the draw: the last thread with mass that starts at or before it -- exactly one thread, however the prefixes
+  // of neighbouring chunks are rounded (NaN mass: none)
+  const float owner = block_max_f(loc > 0.f && rel >= 0.0 ? (float)threadIdx.x : -1.f, red);
+  if ((float)threadIdx.x == owner) {
+    // walk the chunk from 0: an fp32 sum started at the prefix (~ total) would not move for a tail token
+    const float t_loc = (float)rel;
+    float acc = 0.f;
+    int pick = -1, last = -1;
     visit([&](long long i, float x, unsigned short bb) {
       if (pick < 0 && x == x && key16(bb) >= tau) {
-        acc += prob(x);
-        last = i;
-        if (target < acc) pick = (int)i;
+        const float p = prob(x);
+        if (p > 0.f) {
+          acc += p;
+          last = (int)i;
+          if (t_loc < acc) pick = (int)i;
+        }
       }
     });
-    if (pick < 0) pick = (int)last;                                          // rounding at the chunk's upper edge
-    winner_s = pick;
+    winner_s = pick >= 0 ? pick : last;                                      // rounding left the walk short: the last token WITH mass
   }
   __syncthreads();
   if (threadIdx.x == 0) {
     int tok = winner_s;
-    if (tok < 0) {                                                           // target fell into a rounding gap between chunks
-      float best = -INFINITY;                                                // -> most probable token (thread 0 scans the row)
+    if (tok < 0) {                                                           // no usable mass (total 0 or NaN: no finite logit, or +inf)
+      float best = -INFINITY;                                                // -> the first maximum, index 0 if none, as greedy
       for (long long i = 0; i < vocab; ++i) {
         const float x = DT<T>::to_f(row[i]);
         if (x > best) { best = x; tok = (int)i; }

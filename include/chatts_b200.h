@@ -212,6 +212,7 @@ int cts_greedy_advance(cts_ctx* ctx, const void* logits, long long vocab, int ba
  *   top_k > 0: the k largest (ties at the k-th value kept); 0 < top_p < 1: the smallest threshold set whose probability reaches
  *   top_p of the top-k mass.  The token is drawn by inverse CDF in index order with the counter-based uniform
  *   u = splitmix64(seed ^ splitmix64(step << 32 | sequence)) >> 40 / 2^24: (seed, step, sequence) fixes the draw.
+ *   A token of probability 0 (a -inf logit) is never returned; a row without a finite logit gives cts_greedy_advance's token.
  *   temperature > 0 (greedy is cts_greedy_advance); vocab <= 2^24; state pointers as in cts_greedy_advance. */
 int cts_sample_advance(cts_ctx* ctx, const void* logits, long long vocab, int batch, float temperature, int top_k, float top_p,
                        unsigned long long seed, int* out_tokens, int out_ld, int* step_ptr, int* cur_ids, int* positions,
