@@ -14,11 +14,13 @@ between two replays by rewriting its slot's few integers:
 
 Greedy decoding; per-row arithmetic does not depend on the other rows, so a request produces the tokens a stand-alone
 ``generate()`` call produces.  A request may carry vLLM's logits processors (chatts_b200.logit_proc), one parameter set per slot: a
-round in which some active slot uses them runs each step as the decode step without its advance, cts_logit_proc_apply over every slot
-(neutral and free slots are skipped), the greedy advance and cts_logit_proc_update; a round in which none does replays the plain graph.  Host logic only (torch copies of a few int32 per slot); every number comes from the kernels.
+round in which some active slot uses them runs each step as the decode step without its advance followed by the stages of
+chatts_b200.token_pipeline (neutral and free slots are skipped); a round in which none does replays the plain graph.  Host logic only
+(torch copies of a few int32 per slot); every number comes from the kernels.
 """
 from collections import deque
 from dataclasses import dataclass, field
+from types import SimpleNamespace
 
 import numpy as np
 import torch
@@ -26,6 +28,7 @@ import torch
 from . import logit_proc as lpmodp
 from . import logprobs as lpmod
 from ._cabi import LOGPROBS_MAX_K
+from .token_pipeline import TokenPipeline, stop_ids
 
 
 @dataclass
@@ -83,8 +86,7 @@ class ContinuousEngine:
         cfg = self.m.config
         procs = lpmodp.resolve(presence_penalty, frequency_penalty, repetition_penalty, logit_bias, allowed_token_ids, min_tokens,
                                max_new_tokens, vocab=cfg.vocab_size)
-        eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
-        eos = set(eos) if isinstance(eos, (list, tuple, set)) else {int(eos)}
+        eos = stop_ids(eos_token_id, cfg.eos_token_id)
         lpmodp.check_stop_ids(procs, [] if ignore_eos else eos)
         ids = torch.as_tensor(input_ids, dtype=torch.long).reshape(-1)
         ts = series if series is not None else torch.zeros(0, 0, 1)
@@ -179,39 +181,30 @@ class ContinuousEngine:
                 continue
             logits = m._prefill(lay, counts, ts, pts, cached=cached)
             m._prefix_register(keys, pts, lay.lens, cached)
-            # first token + advanced per-sequence state through the greedy kernel on a group-sized scratch state
+            # first token + advanced per-sequence state through the pipeline on a group-sized scratch state, processor rows = the slots
+            # taken.  A row without processors maps to a free slot, whose parameters are neutral (never set, or reset by _release):
+            # the apply kernel returns at once for it.
             g = len(group)
             dev = m.device
             lens32 = torch.from_numpy(lay.lens.astype(np.int32)).to(dev)
-            t_out = torch.zeros(g, 1, dtype=torch.int32, device=dev)
-            t_step = torch.zeros(2, dtype=torch.int32, device=dev)
-            t_cur = torch.zeros(g, dtype=torch.int32, device=dev)
-            t_pos, t_seq = lens32 - 1, lens32.clone()
-            t_slot = torch.zeros(g, dtype=torch.int32, device=dev)
-            t_pt = torch.from_numpy(pts).to(dev)
-            pslots = [free[i] for i, r in enumerate(group) if r.procs is not None]
-            if pslots:                                     # the group's processors, on the first token's (prefill) logits
-                self._set_procs([r for r in group if r.procs is not None], pslots)
-                rows = [i for i, r in enumerate(group) if r.procs is not None]
-                sub = logits[rows]
-                self._proc.apply_rows(sub, pslots)
-                logits[rows] = sub
-            m.ctx.greedy_advance(logits, g, t_out, t_step, t_cur, t_pos, t_seq, t_slot, t_pt, m.page_size)
-            if pslots:
-                cur = torch.full((self.B,), -1, dtype=torch.int32, device=dev)      # -1: rows the update leaves alone
-                cur[torch.tensor(pslots, device=dev)] = t_cur[torch.tensor(rows, device=dev)]
-                self._proc.update(cur, self.B)
+            i32 = dict(dtype=torch.int32, device=dev)
+            t = SimpleNamespace(out_tokens=torch.zeros(g, 1, **i32), step_ptr=torch.zeros(2, **i32), cur_ids=torch.zeros(g, **i32),
+                                positions=lens32 - 1, seq_lens=lens32.clone(), slot_map=torch.zeros(g, **i32),
+                                page_table=torch.from_numpy(pts).to(dev))
+            prows = [i for i, r in enumerate(group) if r.procs is not None]
+            if prows:
+                self._set_procs([group[i] for i in prows], [free[i] for i in prows])
             ks = [r.logprobs for r in group if r.logprobs is not None]
-            if ks:                                         # the first token's logprobs, from the prefill logits
-                lpb = lpmod.LogprobBuffers(m.ctx, g, 1, max(ks), m.config.vocab_size, dev)
-                lpb.launch(logits, g, t_out, step_ptr=t_step)
-            first = t_out[:, 0].cpu().tolist()             # host read: the request's first token (and EOS check)
+            lpb = lpmod.LogprobBuffers(m.ctx, g, 1, max(ks), m.config.vocab_size, dev) if ks else None
+            TokenPipeline(m.ctx, t, g, m.page_size, processors=self._proc if prows else None, slots=free[:g],
+                          logprobs=(lpb, max(ks)) if ks else None).step(logits)
+            first = t.out_tokens[:, 0].cpu().tolist()           # host read: the request's first token (and EOS check)
             if ks:
                 first_lp = lpb.host(1)
             slots = torch.tensor(free[:g], device=dev)
             st = self.st
-            st.cur_ids[slots], st.positions[slots], st.seq_lens[slots], st.slot_map[slots] = t_cur, t_pos, t_seq, t_slot
-            st.page_table[slots] = t_pt
+            st.cur_ids[slots], st.positions[slots], st.seq_lens[slots], st.slot_map[slots] = t.cur_ids, t.positions, t.seq_lens, t.slot_map
+            st.page_table[slots] = t.page_table
             for i, r in enumerate(group):
                 need = (int(lay.lens[i]) + max(q.max_new_tokens for q in group) + self.k + m.page_size - 1) // m.page_size
                 r.pages = [int(x) for x in pts[i, :need]]
@@ -263,17 +256,11 @@ class ContinuousEngine:
         if ks and self._lpb is None:
             self._lpb = lpmod.LogprobBuffers(m.ctx, self.B, self.k, LOGPROBS_MAX_K, m.config.vocab_size, m.device)
         procs = any(r.procs is not None for r in self.active.values())
+        pipe = TokenPipeline(m.ctx, st, self.B, m.page_size, processors=self._proc if procs else None,
+                             logprobs=(self._lpb, max(ks)) if ks else None)          # logprobs: all slots at the largest k asked
         for _ in range(self.k):
-            if procs:
-                m._decode_step(st, sample=False)
-                self._proc.apply(st.full_logits, self.B)
-                m.ctx.greedy_advance(st.full_logits, self.B, st.out_tokens, st.step_ptr, st.cur_ids, st.positions, st.seq_lens, st.slot_map,
-                                     st.page_table, m.page_size)
-                self._proc.update(st.cur_ids, self.B)
-            else:
-                m._decode_step(st, sample=True)
-            if ks:                                         # all slots at the largest k asked; columns from step_ptr
-                self._lpb.launch(st.full_logits, self.B, st.out_tokens, k=max(ks), step_ptr=st.step_ptr)
+            m._decode_step(st, sample=pipe.fused)
+            pipe.step()
         toks = st.out_tokens[:, : self.k].cpu().numpy()    # the round's one device->host read
         lps = self._lpb.host(self.k, max(ks)) if ks else None
         self.occupancy.append(len(self.active))

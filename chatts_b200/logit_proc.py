@@ -188,17 +188,35 @@ class LogitProcState:
         """Occurrence bits of the prompt ids (int32 device tensors) for the repetition penalty."""
         self.ctx.rep_penalty_mark(tokens, rows, self.seen, self.V)
 
-    def apply(self, logits, batch):
-        self.ctx.logit_proc_apply(logits, batch, self.rep, self.presence, self.frequency, self.seen, self.counts, self.bias, self.bias_row,
-                                  self.n_generated, self.min_tokens, self.stop_ids, vocab=self.V)
+    def apply(self, logits, batch, slots=None):
+        """Processors over logits rows [0, batch); ``slots``: logits row i belongs to state row slots[i] (default: row i)."""
+        ix = None if slots is None else torch.as_tensor(slots, dtype=torch.long, device=self.dev)
+        at = lambda t: t if ix is None or t is None else t[ix]
+        self.ctx.logit_proc_apply(logits, batch, at(self.rep), at(self.presence), at(self.frequency), at(self.seen), at(self.counts),
+                                  self.bias, at(self.bias_row), at(self.n_generated), at(self.min_tokens), at(self.stop_ids), vocab=self.V)
 
-    def apply_rows(self, logits, idx):
-        """Apply to logits [len(idx), >= V] whose row i belongs to row idx[i], before any token of those rows is generated (their counts
-        are zero, so none are read)."""
-        ix = torch.as_tensor(idx, dtype=torch.long, device=self.dev)
-        self.ctx.logit_proc_apply(logits, len(idx), self.rep[ix], self.presence[ix], self.frequency[ix], self.seen[ix], None, self.bias,
-                                  self.bias_row[ix], self.n_generated[ix], self.min_tokens[ix],
-                                  self.stop_ids[ix] if self.stop_ids is not None else None, vocab=self.V)
+    def update(self, cur_ids, batch, slots=None):
+        """Counts the new tokens cur_ids[:batch]; ``slots`` as in apply (every other row gets -1, which the kernel leaves alone)."""
+        if slots is not None:
+            cur = torch.full((self.rows,), -1, dtype=torch.int32, device=self.dev)
+            cur[torch.as_tensor(slots, dtype=torch.long, device=self.dev)] = cur_ids[:batch]
+            cur_ids, batch = cur, self.rows
+        self.ctx.logit_proc_update(cur_ids, batch, self.seen, self.counts, self.n_generated, self.V)
+
+
+class RepetitionPenaltyState:
+    """repetition_penalty alone, one value for every row, with LogitProcState's interface: the occurrence bits of the prompt and
+    generated ids, applied by cts_rep_penalty_apply, which touches only the marked ids where cts_logit_proc_apply reads every logit."""
+
+    def __init__(self, ctx, rows, vocab, penalty, device):
+        self.ctx, self.V, self.penalty = ctx, int(vocab), float(penalty)
+        self.seen = torch.zeros(rows, (vocab + 31) // 32, dtype=torch.int32, device=device)
+
+    def mark_prompt(self, tokens, rows):
+        self.ctx.rep_penalty_mark(tokens, rows, self.seen, self.V)
+
+    def apply(self, logits, batch):
+        self.ctx.rep_penalty_apply(logits, batch, self.seen, self.penalty)
 
     def update(self, cur_ids, batch):
-        self.ctx.logit_proc_update(cur_ids, batch, self.seen, self.counts, self.n_generated, self.V)
+        self.ctx.rep_penalty_mark(cur_ids, None, self.seen, self.V)

@@ -57,15 +57,13 @@ class LogprobBuffers:
         n = self.rows * self.cols * k
         return self.ids[:n].view(self.rows, self.cols, k), self.vals[:n].view(self.rows, self.cols, k)
 
-    def launch(self, logits, rows, chosen, k=None, step_ptr=None, col=None, row0=0):
+    def launch(self, logits, rows, chosen, k=None, step_ptr=None, row0=0):
         """Entries of rows [row0, row0 + rows) from logits [rows, >= vocab]: at column step_ptr[0] - 1 (the column the advance just
-        wrote), or at ``col`` of ``chosen`` and of the outputs."""
+        wrote), or at column 0 without step_ptr."""
         k = self.k if k is None else k
         ids, vals = self.topk_views(k)
         lp, rank = self.lp[row0:], self.rank[row0:]
         ids, vals = ids[row0:], vals[row0:]
-        if col is not None:
-            chosen, lp, rank, ids, vals = chosen[:, col:], lp[:, col:], rank[:, col:], ids[:, col:], vals[:, col:]
         self.ctx.logprobs(logits, rows, chosen, k, lp, rank, ids, vals, self.ws, self.counters, step_ptr=step_ptr, vocab=self.vocab)
 
     def host(self, cols, k=None):

@@ -17,10 +17,10 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from . import _cabi, layout, prefix_cache, structured
+from . import _cabi, layout, prefix_cache
 from . import beam as beammod
-from . import logit_proc as lpmodp
 from . import logprobs as lpmod
+from .token_pipeline import TokenPipeline, generate_processors, resolve_generate
 from .trace import span
 from ._cabi import EPI_NONE, EPI_PARTIAL_F32, EPI_RESIDUAL, EPI_SWIGLU_IL
 from .config import ChatTSConfig
@@ -76,7 +76,7 @@ class _Step:
 class ChatTSForCausalLM:
     def __init__(self, config, state_dict, device="cuda", dtype=torch.bfloat16, tp_rank=0, tp_size=1,
                  max_batch=32, max_seq_len=2048, page_size=64, use_cuda_graph=True, comm=None,
-                 use_peer_allreduce=True, graph_with_tp=True, use_chain=None, use_sample_kernel=None, use_native_step=None, use_fused_decode=None, use_peer_ll=None,
+                 use_peer_allreduce=True, graph_with_tp=True, use_chain=None, use_native_step=None, use_fused_decode=None, use_peer_ll=None,
                  enable_prefix_caching=False):
         if enable_prefix_caching and tp_size > 1:
             raise ValueError("enable_prefix_caching is single-GPU only (tensor_parallel_size must be 1)")
@@ -120,10 +120,6 @@ class ChatTSForCausalLM:
                 self._nccl = str(torch.distributed.get_backend(comm)) == "nccl"   # comm None = the default group; gloo (CPU tests) has no reduce_scatter: fp32 all-reduce there
             except Exception:
                 self._nccl = False
-        # sampled decoding through cts_sample_advance (csrc/sampling.cu): temperature / top-k / top-p / multinomial / advance in ONE
-        # launch per step, no torch op on the path (checked against a CPU statement that is itself checked
-        # against transformers' logits warpers).  The default; CTS_SAMPLE_KERNEL=0 selects the torch-op fallback.
-        self.use_sample_kernel = bool(int(_os.environ.get("CTS_SAMPLE_KERNEL", "1"))) if use_sample_kernel is None else bool(use_sample_kernel)
         # bytes of the NEXT GEMM's weight a decode GEMM prefetches into L2 once its own stream is requested.  OFF by default: the
         # prefetched lines do not survive the current GEMM's stream through L2, so the bytes are read twice.  CTS_NEXT_PREFETCH_MB=<n> turns it on for experiments.
         self.next_prefetch_bytes = int(float(_os.environ.get("CTS_NEXT_PREFETCH_MB", "0")) * (1 << 20))
@@ -1117,9 +1113,8 @@ class ChatTSForCausalLM:
 
         structured_outputs = StructuredOutputsParams or {"choice": [...]} / {"regex": "..."}: every row's output is one of the choices,
         or a full match of the regex (chatts_b200.structured), with ``tokenizer`` giving the bytes of each token id (None: ids < 256 are
-        bytes, as SimpleTokenizer encodes).  Each step, the logits of the tokens the automaton does not allow become -inf before the
-        repetition penalty and the greedy or sampled pick, and the logprobs describe that masked distribution; the stop ids are allowed
-        exactly where the output is complete.  If max_new_tokens runs out first, the output is cut there.  Not with ignore_eos; single
+        bytes, as SimpleTokenizer encodes).  Each step, the logits of the tokens the automaton does not allow become -inf, and the logprobs
+        describe that masked distribution; the stop ids are allowed exactly where the output is complete.  If max_new_tokens runs out first, the output is cut there.  Not with ignore_eos; single
         GPU only.
 
         num_beams > 1: beam search with transformers' semantics (chatts_b200.beam), ``length_penalty``, ``early_stopping`` (True, False or
@@ -1130,182 +1125,49 @@ class ChatTSForCausalLM:
 
         presence_penalty, frequency_penalty (each in [-2, 2]), logit_bias ({token id: bias}, clamped to [-100, 100]), allowed_token_ids
         and min_new_tokens (vLLM's min_tokens: the stop ids are refused until a row has generated that many tokens): vLLM's logits
-        processors, applied every step by cts_logit_proc_apply (chatts_b200.logit_proc states the order), together with
-        repetition_penalty, after the structured-output mask and before temperature, top-k and top-p; the logprobs describe the
-        processed logits.  Not with beam search or tensor parallelism; allowed_token_ids and min_new_tokens not with
-        structured_outputs."""
-        cfg, dev = self.config, self.device
-        lpk, plk = lpmod.check_k(logprobs, "logprobs"), lpmod.check_k(prompt_logprobs, "prompt_logprobs")
-        if (lpk is not None or plk is not None) and self.tp_size > 1:
-            raise ValueError("logprobs / prompt_logprobs are single-GPU only (tensor_parallel_size must be 1)")
-        so = structured.resolve(structured_outputs)
-        if so is not None and self.tp_size > 1:
-            raise ValueError("structured_outputs are single-GPU only (tensor_parallel_size must be 1)")
-        if so is not None and ignore_eos:
-            raise ValueError("structured_outputs end the output with a stop id: they cannot be combined with ignore_eos")
-        procs = lpmodp.resolve(presence_penalty, frequency_penalty, None, logit_bias, allowed_token_ids, min_new_tokens,
-                               vocab=cfg.vocab_size)
-        if procs is not None:
-            if num_beams not in (None, 1):
-                raise ValueError("presence_penalty, frequency_penalty, logit_bias, allowed_token_ids and min_new_tokens do not work with "
-                                 "beam search (num_beams > 1)")
-            if self.tp_size > 1:
-                raise ValueError("logits processors are single-GPU only (tensor_parallel_size must be 1)")
-            if so is not None and (procs.allowed_token_ids is not None or procs.min_tokens > 0):
-                raise ValueError("allowed_token_ids and min_new_tokens cannot be combined with structured_outputs: either can refuse "
-                                 "every token the automaton allows")
-        self.last_logprobs = None
-        gd = getattr(self, "generation_defaults", None)
-        if gd:                                          # checkpoint defaults apply only where the caller said nothing
-            if do_sample is None and gd.get("do_sample"):
-                do_sample = True
-                temperature = gd.get("temperature", 1.0) if temperature is None else temperature
-                top_p = gd.get("top_p") if top_p is None else top_p
-                top_k = gd.get("top_k") if top_k is None else top_k
-            if eos_token_id is None and gd.get("eos_token_id") is not None:
-                eos_token_id = gd["eos_token_id"]
-            if pad_token_id is None and gd.get("pad_token_id") is not None:
-                pad_token_id = gd["pad_token_id"]
-            if max_new_tokens is None and max_length is None and gd.get("max_new_tokens"):
-                max_new_tokens = gd["max_new_tokens"]
-            if repetition_penalty is None and gd.get("repetition_penalty") is not None:
-                repetition_penalty = gd["repetition_penalty"]
-        self.last_beam_scores = None
-        if num_beams not in (None, 1):
-            eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
-            eos_ids = [] if ignore_eos else sorted({int(e) for e in (eos if isinstance(eos, (list, tuple, set)) else [eos])})
-            shape = torch.as_tensor(input_ids).shape
-            B = int(shape[0]) if len(shape) > 1 else 1
-            keep = beammod.check_args(num_beams, length_penalty, early_stopping, num_return_sequences, len(eos_ids), B, self.max_batch,
-                                      do_sample=do_sample, num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty,
-                                      repetition_penalty=repetition_penalty, logprobs=logprobs, prompt_logprobs=prompt_logprobs,
-                                      structured_outputs=structured_outputs, streamer=streamer, tp_size=self.tp_size)
-            return self._beam_generate(input_ids, attention_mask, timeseries, max_new_tokens, max_length, eos_ids,
-                                       cfg.pad_token_id if pad_token_id is None else pad_token_id, int(num_beams), keep, length_penalty,
-                                       early_stopping, int(num_return_sequences), sync_every)
+        processors, applied every step together with repetition_penalty (chatts_b200.logit_proc states their order); the logprobs
+        describe the processed logits.  Not with beam search or tensor parallelism; allowed_token_ids and min_new_tokens not with
+        structured_outputs.  chatts_b200.token_pipeline states the order of the per-step stages."""
+        o = resolve_generate(self, input_ids, max_new_tokens=max_new_tokens, max_length=max_length, do_sample=do_sample,
+                             temperature=temperature, top_p=top_p, top_k=top_k, streamer=streamer, eos_token_id=eos_token_id,
+                             pad_token_id=pad_token_id, ignore_eos=ignore_eos, seed=seed, repetition_penalty=repetition_penalty,
+                             logprobs=logprobs, prompt_logprobs=prompt_logprobs, structured_outputs=structured_outputs, tokenizer=tokenizer,
+                             num_beams=num_beams, length_penalty=length_penalty, early_stopping=early_stopping,
+                             num_return_sequences=num_return_sequences, num_beam_groups=num_beam_groups,
+                             diversity_penalty=diversity_penalty, presence_penalty=presence_penalty, frequency_penalty=frequency_penalty,
+                             logit_bias=logit_bias, allowed_token_ids=allowed_token_ids, min_new_tokens=min_new_tokens)
+        self.last_logprobs = self.last_beam_scores = None
+        if o.beams is not None:
+            return self._beam_generate(input_ids, attention_mask, timeseries, o.max_new_tokens, sorted(o.eos), o.pad, int(num_beams),
+                                       o.beams, length_penalty, early_stopping, int(num_return_sequences), sync_every)
         ids_cpu, am_cpu, counts, lay = self._prepare_inputs(input_ids, attention_mask, timeseries)
         B, S = ids_cpu.shape
-        if max_new_tokens is None:
-            max_new_tokens = (max_length - S) if max_length is not None else 20
-        max_new_tokens = int(max_new_tokens)
+        max_new_tokens, eos_set, V, dev = o.max_new_tokens, o.eos, self.config.vocab_size, self.device
         if max_new_tokens <= 0:
             return torch.as_tensor(ids_cpu, dtype=torch.long)
-        eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
-        eos_set = set(eos) if isinstance(eos, (list, tuple, set)) else {int(eos)}
-        if procs is not None:
-            if procs.min_tokens > max_new_tokens:
-                raise ValueError(f"min_new_tokens ({procs.min_tokens}) must be <= max_new_tokens ({max_new_tokens})")
-            lpmodp.check_stop_ids(procs, [] if ignore_eos else eos_set)
-            rp = repetition_penalty if repetition_penalty is not None else 1.0
-            if not rp > 0:
-                raise ValueError(f"repetition_penalty must be > 0, got {repetition_penalty}")
-            procs.repetition_penalty = float(rp)
-        pad = cfg.pad_token_id if pad_token_id is None else pad_token_id
-        auto = None
-        if so is not None:
-            # compiled (or found in the cache) before any page is taken: a pattern error leaves the pool as it was
-            if getattr(self, "_struct_cache", None) is None:
-                self._struct_cache = structured.AutomatonCache(self.ctx, dev)
-            auto = self._struct_cache.get(so, tokenizer, self.config.vocab_size, eos_set)
-        if do_sample and temperature is None:
-            temperature = 1.0                                   # HF GenerationConfig default when do_sample=True names no temperature
-        greedy = not (do_sample and temperature > 0)
-        if not greedy and seed is None:
-            # an unseeded call draws a fresh seed (a fresh torch.Generator would start from the same default seed every time);
-            # under tensor parallelism rank 0's seed is broadcast so every rank picks the same tokens
-            seed = int.from_bytes(__import__("os").urandom(7), "little")
-            if self.tp_size > 1:
-                box = [seed]
-                torch.distributed.broadcast_object_list(box, src=0, group=self.comm)
-                seed = int(box[0])
-        page_tables, held, keys, cached = self._alloc_prompt(lay, timeseries, max_new_tokens, lookup=plk is None)
+        page_tables, held, keys, cached = self._alloc_prompt(lay, timeseries, max_new_tokens, lookup=o.prompt_logprobs is None)
         try:
             with span("cts.prefill"):
-                logits = self._prefill(lay, counts, timeseries, page_tables, cached=cached, prompt_lp=plk)
+                logits = self._prefill(lay, counts, timeseries, page_tables, cached=cached, prompt_lp=o.prompt_logprobs)
             plp = None
-            if plk is not None:
+            if o.prompt_logprobs is not None:
                 logits, plp = logits
             self._prefix_register(keys, page_tables, lay.lens, cached)
             self.last_cached_positions = cached          # per row: prompt positions whose KV came from the prefix cache (None: caching off)
             st = self._decode_state(B, max_new_tokens)
             lens32 = torch.from_numpy(lay.lens.astype(np.int32))
             st.page_table.copy_(torch.from_numpy(page_tables), non_blocking=True)
-            st.positions.copy_(lens32 - 1, non_blocking=True)       # advanced to len by the first greedy_advance
+            st.positions.copy_(lens32 - 1, non_blocking=True)       # advanced to len by the first token's advance
             st.seq_lens.copy_(lens32, non_blocking=True)             # -> len + 1: cache length once the new token is written
             st.step_ptr.zero_()
-            gen = torch.Generator(device=dev)
-            if seed is not None:
-                gen.manual_seed(int(seed))
-            kseed = int(seed) if seed is not None else 0
-            # structured outputs: each row's automaton state lives on the device next to cur_ids; every step masks the logits by it
-            # before anything reads them and walks it over the picked token after the advance
-            struct_state = None
-            if auto is not None:
-                struct_state = torch.zeros(B, dtype=torch.int32, device=dev)
-                auto.mask_apply(self.ctx, logits, B, struct_state)
-
-            def sample(lg, step):
-                if self.use_sample_kernel:
-                    # temperature / top-k / top-p + multinomial + advance in one launch; the draw is a function of (seed, step, row)
-                    self.ctx.sample_advance(lg, B, temperature, top_k or 0, 1.0 if top_p is None else top_p, kseed, st.out_tokens,
-                                            st.step_ptr, st.cur_ids, st.positions, st.seq_lens, st.slot_map, st.page_table,
-                                            self.page_size)
-                else:
-                    self._sample_advance(st, lg, step, temperature, top_p, gen, top_k)
-
-            # repetition penalty (transformers RepetitionPenaltyLogitsProcessor, e.g. from generation_config.json): the ids that occur in
-            # a row -- prompt (the un-expanded input_ids, as HF sees them) and generated -- live in a device bit mask; every step's
-            # logits are rewritten by cts_rep_penalty_apply before the argmax / sampling kernel, the new token is marked after it
-            rep = float(repetition_penalty) if repetition_penalty not in (None, 1, 1.0) else None
-            seen = None
-            proc = None
-            if procs is not None:
-                # every other processor on: cts_logit_proc_apply takes over the repetition penalty, its update marks the new tokens
-                proc = lpmodp.LogitProcState(self.ctx, B, self.config.vocab_size, self.n_pos, dev)
-                proc.set_rows(list(range(B)), procs, [] if ignore_eos else eos_set, shared_bias=True)
-                if rep is not None:
-                    am = np.ones_like(ids_cpu) if am_cpu is None else am_cpu
-                    rr, cc = np.nonzero(am)
-                    proc.mark_prompt(torch.from_numpy(ids_cpu[rr, cc].astype(np.int32)).to(dev), torch.from_numpy(rr.astype(np.int32)).to(dev))
-                proc.apply(logits, B)
-            elif rep is not None:
-                Vfull = self.config.vocab_size
-                seen = torch.zeros(B, (Vfull + 31) // 32, dtype=torch.int32, device=dev)
-                am = np.ones_like(ids_cpu) if am_cpu is None else am_cpu
-                rr, cc = np.nonzero(am)
-                self.ctx.rep_penalty_mark(torch.from_numpy(ids_cpu[rr, cc].astype(np.int32)).to(dev), torch.from_numpy(rr.astype(np.int32)).to(dev),
-                                          seen, Vfull)
-                self.ctx.rep_penalty_apply(logits, B, seen, rep)
-
-            def advance(lg, step):
-                if greedy:
-                    self.ctx.greedy_advance(lg, B, st.out_tokens, st.step_ptr, st.cur_ids, st.positions, st.seq_lens, st.slot_map,
-                                            st.page_table, self.page_size)
-                else:
-                    sample(lg, step)
-                if proc is not None:
-                    proc.update(st.cur_ids, B)
-                elif seen is not None:
-                    self.ctx.rep_penalty_mark(st.cur_ids, None, seen, self.config.vocab_size)
-                if auto is not None:
-                    auto.advance(self.ctx, st.cur_ids, B, struct_state)
-
-            # logprobs: one cts_logprobs launch after each advance, over the logits the token was picked from; the kernel advances
-            # (greedy, sample) leave step_ptr one past the column they wrote, the torch sampler does not move it.  Only called when
-            # asked: under tensor parallelism (refused above) the vocab-parallel greedy step leaves no full_logits.
-            lpb = None if lpk is None else lpmod.LogprobBuffers(self.ctx, B, max_new_tokens, lpk, self.config.vocab_size, dev)
-
-            def take_logprobs(lg, step):
-                if greedy or self.use_sample_kernel:
-                    lpb.launch(lg, B, st.out_tokens, step_ptr=st.step_ptr)
-                else:
-                    lpb.launch(lg, B, st.out_tokens, col=step)
-
-            advance(logits, 0)
-            if lpb is not None:
-                take_logprobs(logits, 0)
+            pipe = TokenPipeline(
+                self.ctx, st, B, self.page_size, sampling=o.sampling,
+                automaton=None if o.automaton is None else (o.automaton, torch.zeros(B, dtype=torch.int32, device=dev)),
+                processors=generate_processors(self.ctx, o.procs, ids_cpu, am_cpu, eos_set, V, self.n_pos, dev),
+                logprobs=None if o.logprobs is None else (lpmod.LogprobBuffers(self.ctx, B, max_new_tokens, o.logprobs, V, dev), o.logprobs))
+            pipe.step(logits)
             done = np.zeros(B, dtype=bool)
-            out = np.full((B, max_new_tokens), pad, dtype=np.int64)
+            out = np.full((B, max_new_tokens), o.pad, dtype=np.int64)
             emitted = 0
             produced = 1
             chunk = 1 if streamer is not None else max(1, int(sync_every))
@@ -1318,38 +1180,26 @@ class ChatTSForCausalLM:
                         out[~done, emitted + j] = col[~done]
                         if streamer is not None:
                             streamer.put(torch.as_tensor(col))
-                        if not ignore_eos:
-                            done |= np.isin(col, list(eos_set))
+                        done |= np.isin(col, list(eos_set))
                     emitted = produced
                     if produced >= max_new_tokens or done.all():
                         break
                 with span("cts.decode_step"):
-                    if greedy and seen is None and auto is None and proc is None:
-                        self._decode_step(st, sample=True)
-                    else:
-                        self._decode_step(st, sample=False)
-                        if auto is not None:
-                            auto.mask_apply(self.ctx, st.full_logits, B, struct_state)
-                        if proc is not None:
-                            proc.apply(st.full_logits, B)
-                        elif seen is not None:
-                            self.ctx.rep_penalty_apply(st.full_logits, B, seen, rep)
-                        advance(st.full_logits, produced)
-                    if lpb is not None:
-                        take_logprobs(st.full_logits, produced)
+                    self._decode_step(st, sample=pipe.fused)
+                    pipe.step()
                 produced += 1
             if streamer is not None:
                 streamer.end()
         finally:
             self.pool.release(held)
-        is_eos = np.isin(out[:, :emitted], list(eos_set)) if not ignore_eos else np.zeros((B, emitted), dtype=bool)
+        is_eos = np.isin(out[:, :emitted], list(eos_set))
         first = np.where(is_eos.any(axis=1), is_eos.argmax(axis=1) + 1, emitted)
         n_out = int(min(max(first.max(), 1), max_new_tokens))
-        if lpk is not None or plk is not None:
+        if o.logprobs is not None or o.prompt_logprobs is not None:
             res = lpmod.GenerationLogprobs()
-            if lpb is not None:
-                res.logprobs, res.ranks, res.top_ids, res.top_logprobs = lpb.host(n_out)
-                if auto is not None:                      # a token the constraint refused has probability 0: an empty top-k slot
+            if pipe.lpb is not None:
+                res.logprobs, res.ranks, res.top_ids, res.top_logprobs = pipe.lpb.host(n_out)
+                if o.automaton is not None:               # a token the constraint refused has probability 0: an empty top-k slot
                     gone = np.isneginf(res.top_logprobs)
                     res.top_ids[gone], res.top_logprobs[gone] = -1, np.nan
             if plp is not None:
@@ -1358,17 +1208,14 @@ class ChatTSForCausalLM:
             self.last_logprobs = res
         return torch.cat([torch.as_tensor(ids_cpu, dtype=torch.long), torch.as_tensor(out[:, :n_out])], dim=1)
 
-    def _beam_generate(self, input_ids, attention_mask, timeseries, max_new_tokens, max_length, eos_ids, pad, nb, keep, length_penalty,
-                       early_stopping, nrs, sync_every):
+    def _beam_generate(self, input_ids, attention_mask, timeseries, max_new, eos_ids, pad, nb, keep, length_penalty, early_stopping, nrs,
+                       sync_every):
         """Beam search (see generate): one prefill per prompt, then every step the decode step of the B * nb beam rows (graph replay
         without the advance), cts_logprobs for each row's top ``keep`` candidates, cts_beam_select and cts_beam_fork_kv, all on one
         stream; the host reads the per-prompt done flags every ``sync_every`` steps and walks the back-pointers once at the end."""
         c, dev, ps = self.ctx, self.device, self.page_size
         ids_cpu, am_cpu, counts, lay = self._prepare_inputs(input_ids, attention_mask, timeseries)
         B, S = ids_cpu.shape
-        if max_new_tokens is None:
-            max_new_tokens = (max_length - S) if max_length is not None else 20
-        max_new = int(max_new_tokens)
         if max_new <= 0:
             return torch.as_tensor(ids_cpu, dtype=torch.long).repeat_interleave(nrs, 0)
         R, V = B * nb, self.config.vocab_size
@@ -1443,27 +1290,3 @@ class ChatTSForCausalLM:
             out[r, S:S + len(h)] = h
         self.last_beam_scores = torch.from_numpy(np.stack([scores[b * nb:b * nb + nrs] for b in range(B)]).reshape(-1).copy())
         return torch.from_numpy(out)
-
-    def _sample_advance(self, st, logits, step, temperature, top_p, gen, top_k=None):
-        """Stochastic sampling (temperature / top-p, chatts/utils/inference_tsmllm_deepspeed.py:95-100).  Round 1: the
-        distribution arithmetic is torch on the device logits (not graph-captured); greedy is the fused kernel."""
-        lg = logits[: st.B].float() / float(temperature)
-        if top_k is not None and 0 < top_k < lg.shape[-1]:
-            kth = torch.topk(lg, int(top_k), dim=-1).values[:, -1:]
-            lg = lg.masked_fill(lg < kth, float("-inf"))
-        probs = torch.softmax(lg, dim=-1)
-        if top_p is not None and top_p < 1.0:
-            sp, si = torch.sort(probs, dim=-1, descending=True)
-            keep = (torch.cumsum(sp, dim=-1) - sp) < top_p
-            sp = sp * keep
-            probs = torch.zeros_like(probs).scatter_(1, si, sp)
-            probs = probs / probs.sum(dim=-1, keepdim=True)
-        tok = torch.multinomial(probs, 1, generator=gen).reshape(-1).to(torch.int32)
-        st.out_tokens[:, step] = tok
-        st.cur_ids.copy_(tok)
-        st.positions.add_(1)
-        st.seq_lens.add_(1)
-        pg = torch.div(st.positions, self.page_size, rounding_mode="floor").long().clamp_(max=self.max_pages - 1)
-        st.slot_map.copy_((st.page_table.gather(1, pg[:, None]).reshape(-1) * self.page_size +
-                           st.positions % self.page_size).to(torch.int32))
-        st.step_ptr[0] += 1

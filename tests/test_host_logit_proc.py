@@ -199,7 +199,7 @@ def test_refusals_take_nothing(cabi_double):
              (dict(allowed_token_ids=[1], structured_outputs={"choice": ["a"]}), "structured"), (dict(logit_bias={1000: 1}), "vocabulary"),
              (dict(allowed_token_ids=[5, 1001]), "vocabulary"), (dict(min_new_tokens=5), "max_new_tokens"),
              (dict(presence_penalty=2.5), r"\[-2, 2\]"), (dict(min_new_tokens=1, eos_token_id=list(range(65))), "64 stop ids"),
-             (dict(frequency_penalty=0.1, repetition_penalty=0.0), "repetition_penalty")]
+             (dict(frequency_penalty=0.1, repetition_penalty=0.0), "repetition_penalty"), (dict(repetition_penalty=0.0), "repetition_penalty")]
     for kw, match in cases:
         with pytest.raises(ValueError, match=match):
             model.generate(**enc, max_new_tokens=4, **kw)
@@ -257,19 +257,24 @@ def test_engine_matches_generate_and_leaves_neutral_slots_alone(cabi_double):
     _, _, model, proc = _build(cabi_double)
     prompts = ["first prompt", "a second, longer prompt", "third", "fourth one"]
     kws = [dict(), dict(presence_penalty=0.8, frequency_penalty=0.3, repetition_penalty=1.4, logit_bias={101: 3.0}, min_tokens=3),
-           dict(allowed_token_ids=list(range(97, 110)) + [EOS], min_tokens=2), dict()]
+           dict(allowed_token_ids=list(range(97, 110)) + [EOS], min_tokens=2), dict(logprobs=2)]
     gen_kw = lambda kw: {("min_new_tokens" if k == "min_tokens" else k): v for k, v in kw.items()}
-    want = []
+    want, want_lp = [], []
     for p, kw in zip(prompts, kws):
         enc = _enc(proc, [p])
         S = enc["input_ids"].shape[1]
         want.append(model.generate(**enc, max_new_tokens=9, **gen_kw(kw))[0, S:].tolist())
+        want_lp.append(model.last_logprobs)
     eng = ContinuousEngine(model, slots=4, steps_per_round=3)
     rids = [eng.add_request(_enc(proc, [p])["input_ids"][0], max_new_tokens=9, **kw) for p, kw in zip(prompts, kws)]
     done = {r.rid: r for r in eng.run()}
     for rid, w in zip(rids, want):
         toks = done[rid].tokens
         assert toks == w[:len(toks)] and (len(toks) == 9 or toks[-1] == EOS), (toks, w)
+    lp = want_lp[3]                                         # the logprobs request, in a round with a processors request and a plain one
+    got = done[rids[3]].token_logprobs
+    assert len(got) == len(done[rids[3]].tokens) and got == [
+        (float(lp.logprobs[0, j]), int(lp.ranks[0, j]), lp.top_ids[0, j].tolist(), lp.top_logprobs[0, j].tolist()) for j in range(len(got))]
     assert not eng._proc.min_tokens.any() and bool((eng._proc.bias_row == -1).all()) and bool((eng._proc.rep == 1).all())
     eng.close()
     assert model.pool.available() == model.pool.num_pages

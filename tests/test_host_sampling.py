@@ -1,6 +1,6 @@
 """Sampled decoding (temperature / top-k / top-p) on CPU: the statement cts_sample_advance follows (tests/cabi_double.py
 ``sample_reference``: threshold sets by bisection over the 16-bit logit key, inverse CDF in index order, counter-based
-uniform) against transformers' own logits warpers, and generate(do_sample=True, use_sample_kernel=True) through the
+uniform) against transformers' own logits warpers, and generate(do_sample=True) through the
 double: reproducible per seed, top_k=1 == greedy, every token inside the kept set."""
 import numpy as np
 import pytest
@@ -46,8 +46,8 @@ def test_uniform_stream_is_uniform_and_reproducible():
     assert len(set(u.tolist())) > 1590
 
 
-def test_generate_with_sampling_kernel(cabi_double):
-    cfg, sd, model, proc = _build(cabi_double, split=1, use_sample_kernel=True)
+def test_generate_samples_through_the_kernel(cabi_double):
+    cfg, sd, model, proc = _build(cabi_double, split=1)
     enc = proc(text=PROMPTS, timeseries=list(_series()), padding=True, return_tensors="pt")
     kw = dict(max_new_tokens=10, do_sample=True, temperature=0.8, top_p=0.9, top_k=40, ignore_eos=True)
     a = model.generate(**enc, seed=5, **kw)
@@ -59,10 +59,6 @@ def test_generate_with_sampling_kernel(cabi_double):
     row = torch.arange(1000, dtype=torch.float32).mul(0.01).to(DT)
     row[417] = 50.0
     assert TorchDouble.sample_reference(row, 1.0, 1, 1.0, seed=3, step=0, b=0)[0] == 417
-    # the torch path (use_sample_kernel=False) accepts the same arguments
-    model.use_sample_kernel = False
-    d = model.generate(**enc, seed=5, **kw)
-    assert d.shape == a.shape
 
 
 def test_repetition_penalty_matches_transformers_processor(cabi_double):

@@ -39,21 +39,24 @@ def main():
     new = int(os.environ.get("TP_CHECK_NEW", "12"))
     tp = ChatTSForCausalLM(cfg, sd, dtype=dt, tp_rank=rank, tp_size=world, max_batch=4, max_seq_len=512, page_size=16)
     lg_tp = tp.forward(enc["input_ids"], enc["attention_mask"], enc["timeseries"]).logits[:, 0].float()
-    ids_tp = tp.generate(**enc, max_new_tokens=new, ignore_eos=True)
+    runs = [dict(), dict(repetition_penalty=1.3)]          # the penalty alone runs on the eager decode step over the gathered logits
+    ids_tp = [tp.generate(**enc, max_new_tokens=new, ignore_eos=True, **kw) for kw in runs]
     ok = True
     if rank == 0:
         ref = ChatTSForCausalLM(cfg, sd, dtype=dt, max_batch=4, max_seq_len=512, page_size=16, use_fused_decode=0)
         lg = ref.forward(enc["input_ids"], enc["attention_mask"], enc["timeseries"]).logits[:, 0].float()
-        ids = ref.generate(**enc, max_new_tokens=new, ignore_eos=True)
+        ids = [ref.generate(**enc, max_new_tokens=new, ignore_eos=True, **kw) for kw in runs]
         err = float((lg_tp - lg).abs().max() / lg.abs().max())
         S = enc["input_ids"].shape[1]
-        agree = [int(next((i for i in range(new) if ids[b, S + i] != ids_tp[b, S + i]), new)) for b in range(2)]
+        agree = [[int(next((i for i in range(new) if a[b, S + i] != t[b, S + i]), new)) for b in range(2)] for a, t in zip(ids, ids_tp)]
         print(f"[shim_tp_check] world={world} peer_ll={int(tp.use_peer_ll)} fused={tp.use_fused_decode} logits rel err vs single rank {err:.3e}; "
-              f"greedy agreement {agree}/{new}", flush=True)
-        ok = err < 2e-2 and min(agree) >= min(new, 4)
-    lst = [torch.empty_like(ids_tp) for _ in range(world)]
-    dist.all_gather(lst, ids_tp)
-    same = all(torch.equal(lst[0], t) for t in lst)
+              f"greedy agreement {agree[0]}/{new}, with repetition_penalty=1.3 {agree[1]}/{new}", flush=True)
+        ok = err < 2e-2 and min(min(a) for a in agree) >= min(new, 4)
+    same = True
+    for t in ids_tp:
+        lst = [torch.empty_like(t) for _ in range(world)]
+        dist.all_gather(lst, t)
+        same = same and all(torch.equal(lst[0], x) for x in lst)
     if rank == 0:
         print(f"[shim_tp_check] identical tokens on all ranks: {same}", flush=True)
     dist.barrier()
