@@ -28,7 +28,7 @@ SYMBOLS = [
     "cts_attn_prefill_lse", "cts_attn_bwd", "cts_swiglu", "cts_swiglu_bwd", "cts_rmsnorm_bwd", "cts_qkv_rope_bwd",
     "cts_ce_loss_grad", "cts_gather_rows", "cts_lora_wgrad", "cts_adamw", "cts_grad_norm_ws_floats", "cts_grad_norm_clip",
     "cts_lora_pack",
-    "cts_sample_advance", "cts_rmsnorm", "cts_lm_head", "cts_decoder_step_ws_floats", "cts_decoder_step", "cts_ts_encode", "cts_gemm_decode_fused",
+    "cts_sample_advance", "cts_sample_advance_rows", "cts_rmsnorm", "cts_lm_head", "cts_decoder_step_ws_floats", "cts_decoder_step", "cts_ts_encode", "cts_gemm_decode_fused",
     "cts_peer_ll_region_bytes", "cts_peer_allreduce_ll", "cts_trace_enable", "cts_ts_encode_fused_ok", "cts_ts_encode_fused",
     "cts_rep_penalty_mark", "cts_rep_penalty_apply", "cts_gemm_w4", "cts_gemm_w4_suggest_split", "cts_gemm_w4_mma", "cts_gemm_w4_mma_suggest_split",
     "cts_gemm_fp8", "cts_gemm_fp8_suggest_split", "cts_fp8_dequant", "cts_attn_prefill_paged",
@@ -201,6 +201,8 @@ def load_library():
         getattr(lib, name).restype = i
     lib.cts_sample_advance.argtypes = [vp, vp, ll, i, f, i, f, C.c_ulonglong, vp, i, vp, vp, vp, vp, vp, vp, i, i, i, vp]
     lib.cts_sample_advance.restype = i
+    lib.cts_sample_advance_rows.argtypes = [vp, vp, ll, i, vp, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, i, i, i, vp]
+    lib.cts_sample_advance_rows.restype = i
     lib.cts_logprobs_workspace_floats.argtypes = [i, ll, i]
     lib.cts_logprobs_workspace_floats.restype = ll
     lib.cts_logprobs.argtypes = [vp, vp, ll, ll, i, vp, i, vp, i, vp, vp, vp, vp, i, vp, vp, i, vp]
@@ -612,6 +614,24 @@ class Context:
                                               _p(positions), _p(seq_lens), _p(slot_map), _p(page_table),
                                               page_table.shape[1] if page_table is not None else 0, page_size,
                                               dtype_code(logits.dtype), _stream()))
+
+    def sample_advance_rows(self, logits, batch, temperature, top_k, top_p, seed, draw_key, draw_step, out_tokens, step_ptr, cur_ids,
+                            positions, seq_lens, slot_map, page_table, page_size):
+        """cts_sample_advance with per-row parameters: temperature float32, top_k int32, top_p float32, seed int64 (read as uint64),
+        draw_key int32 and draw_step int32, each [>= batch]; a row with temperature <= 0 is greedy; draw_step[b] += 1."""
+        if logits.dim() != 2 or logits.shape[0] < batch:
+            raise CtsError(f"sample_advance_rows: expected logits [>= {batch}, V], got {tuple(logits.shape)}")
+        for name, t, dt in (("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32), ("top_p", top_p, torch.float32),
+                            ("seed", seed, torch.int64), ("draw_key", draw_key, torch.int32), ("draw_step", draw_step, torch.int32)):
+            if t is None:
+                raise CtsError(f"sample_advance_rows: {name} is required")
+            _check_rows("sample_advance_rows", batch, [(t, dt, 1)])
+        self._chk(self.lib.cts_sample_advance_rows(self.h, _p(logits), logits.shape[-1], batch, _p(temperature), _p(top_k), _p(top_p),
+                                                   _p(seed), _p(draw_key), _p(draw_step), _p(out_tokens),
+                                                   out_tokens.stride(0) if out_tokens is not None else 0, _p(step_ptr), _p(cur_ids),
+                                                   _p(positions), _p(seq_lens), _p(slot_map), _p(page_table),
+                                                   page_table.shape[1] if page_table is not None else 0, page_size,
+                                                   dtype_code(logits.dtype), _stream()))
 
     def logprobs_workspace_floats(self, rows, vocab, k):
         return int(self.lib.cts_logprobs_workspace_floats(int(rows), int(vocab), int(k)))

@@ -15,7 +15,10 @@
 // behind a dominant one (below ulp(1) of an fp32 prefix) keeps its share.  One block max names the single chunk that holds the
 // target, and that chunk is walked from 0 against the target's offset into it.  Only tokens with mass are ever returned: a -inf
 // logit (a structured-output or allowed-id refusal, a min_tokens stop id) never is.  A row without usable mass (no finite logit)
-// gives cts_greedy_advance's token.
+// gives cts_greedy_advance's token, found by a block-wide argmax.
+// cts_sample_advance_rows runs the same kernel with every parameter read per row (the continuous engine's slots): a row with
+// temperature <= 0 is greedy, and its draw is keyed on the row's own (seed, draw_step, draw_key) rather than (step, CTA index), so a
+// request's tokens do not depend on the slot it occupies or on the round its steps fall in.
 #include "common.cuh"
 
 namespace {
@@ -57,10 +60,54 @@ __device__ __forceinline__ float block_max_f(float v, float* red) {
   return red[0];
 }
 
+// cts_greedy_advance's token of one row for thread 0 (the first maximum, NaN never wins, 0 when no value exceeds -inf): a greedy row,
+// or a sampled one without usable mass.  Kept out of line so that it does not weigh on the sampler's register allocation.
+template <typename T>
+__device__ __attribute__((noinline)) int block_argmax(const T* __restrict__ row, long long vocab, unsigned long long* red) {
+  float best = -INFINITY;
+  long long best_i = vocab;
+  for (long long i = threadIdx.x; i < vocab; i += kSaThreads) {
+    const float x = DT<T>::to_f(row[i]);
+    if (x > best) { best = x; best_i = i; }                                  // strided: the first maximum of this thread's indices
+  }
+  // key = ordered value bits above the complemented index: the block max is the first maximum (-0 and +0 tie)
+  unsigned u = __float_as_uint(best);
+  if ((u << 1) == 0u) u = 0u;
+  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  unsigned long long key = best_i < vocab ? ((unsigned long long)u << 32) | (unsigned)~(unsigned)best_i : 0ull;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long w = __shfl_xor_sync(0xffffffffu, key, o);
+    key = w > key ? w : key;
+  }
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = key;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    key = red[threadIdx.x];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long w = __shfl_xor_sync(0xffffffffu, key, o);
+      key = w > key ? w : key;
+    }
+  }
+  return key ? (int)~(unsigned)key : 0;
+}
+
+// Per-row sampling parameters (cts_sample_advance_rows): each non-null array replaces the launch's scalar for row b, and the draw is
+// u(seed, draw_step[b], draw_key[b]) instead of u(seed, step_ptr[0], b).  All null: cts_sample_advance.
+struct RowParams {
+  const float* temperature;
+  const int* top_k;
+  const float* top_p;
+  const unsigned long long* seed;
+  const int* draw_key;
+  int* draw_step;
+};
+
 template <typename T>
 __global__ void __launch_bounds__(kSaThreads)
 sample_advance_kernel(const T* __restrict__ logits, long long vocab, float inv_temp, int top_k, float top_p, unsigned long long seed,
-                      int* __restrict__ out_tokens, int out_ld, int* __restrict__ step_ptr, int* __restrict__ cur_ids,
+                      RowParams rp, int* __restrict__ out_tokens, int out_ld, int* __restrict__ step_ptr, int* __restrict__ cur_ids,
                       int* __restrict__ positions, int* __restrict__ seq_lens, int* __restrict__ slot_map,
                       const int* __restrict__ page_table, int max_pages, int page_size) {
   pdl_trigger();
@@ -69,7 +116,18 @@ sample_advance_kernel(const T* __restrict__ logits, long long vocab, float inv_t
   __shared__ double scan_s[32];
   __shared__ double total_s;
   __shared__ int winner_s;
+  __shared__ unsigned long long argmax_s[32];
   const int b = blockIdx.x;
+  // a row with temperature <= 0 (or NaN) is greedy
+  bool greedy = false;
+  if (rp.temperature) {
+    const float t = rp.temperature[b];
+    greedy = !(t > 0.f);
+    inv_temp = greedy ? 1.f : 1.0f / t;                                      // IEEE division (no fast math): the host's 1.0f / temperature
+  }
+  if (rp.top_k) top_k = rp.top_k[b];
+  if (rp.top_p) top_p = rp.top_p[b];
+  if (rp.seed) seed = rp.seed[b];
   const T* row = logits + (long long)b * vocab;
   // contiguous chunk of indices per thread (multiple of 8 so the vector path stays aligned)
   const long long per = ((vocab + kSaThreads - 1) / kSaThreads + 7) / 8 * 8;
@@ -91,107 +149,105 @@ sample_advance_kernel(const T* __restrict__ logits, long long vocab, float inv_t
     }
   };
 
-  // ---- max and partition function of z = logit / temperature
-  float m = -INFINITY;
-  visit([&](long long, float x, unsigned short) { if (x > m) m = x; });      // NaN never wins
-  m = block_max_f(m, red);
-  auto prob = [&](float x) { return x == x ? __expf((x - m) * inv_temp) : 0.f; };   // unnormalised; NaN logits get mass 0
-  unsigned kmax = 0;
-  visit([&](long long, float x, unsigned short bb) { if (x == x) { const unsigned k = key16(bb); if (k > kmax) kmax = k; } });
-  kmax = (unsigned)block_max_f((float)kmax, red);                            // keys < 2^16 are exact in fp32
-  auto mass_ge = [&](unsigned tau) {
-    float s = 0.f;
-    visit([&](long long, float x, unsigned short bb) { if (x == x && key16(bb) >= tau) s += prob(x); });
-    return block_sum_f(s, red);
-  };
-  auto count_ge = [&](unsigned tau) {
-    float c = 0.f;
-    visit([&](long long, float x, unsigned short bb) { if (x == x && key16(bb) >= tau) c += 1.f; });
-    return block_sum_f(c, red);                                              // counts <= 2^24 are exact in fp32
-  };
-  unsigned tau = 0;
-  if (top_k > 0 && (long long)top_k < vocab) {
-    unsigned lo = 0, hi = kmax + 1;                                          // count(>= lo) >= k holds, count(>= hi) = 0 does not
-    while (hi - lo > 1) {
-      const unsigned mid = lo + ((hi - lo) >> 1);
-      if (count_ge(mid) >= (float)top_k) lo = mid; else hi = mid;
-    }
-    tau = lo;
-  }
-  float mass = mass_ge(tau);
-  if (top_p > 0.f && top_p < 1.f) {
-    const float target = top_p * mass;
-    unsigned lo = tau, hi = kmax + 1;
-    while (hi - lo > 1) {
-      const unsigned mid = lo + ((hi - lo) >> 1);
-      if (mass_ge(mid) >= target) lo = mid; else hi = mid;
-    }
-    if (lo != tau) { tau = lo; mass = mass_ge(tau); }
-  }
-  // ---- inverse CDF in index order over the kept set
-  const int step = step_ptr ? step_ptr[0] : 0;
-  const unsigned long long h = splitmix64(seed ^ splitmix64(((unsigned long long)(unsigned)step << 32) | (unsigned)b));
-  const double u = (double)(h >> 40) * (1.0 / 16777216.0);                  // 24 random bits -> [0, 1)
-  float loc = 0.f;
-  visit([&](long long, float x, unsigned short bb) { if (x == x && key16(bb) >= tau) loc += prob(x); });
-  // block exclusive scan of the per-thread sums (threads own increasing index ranges), in fp64: in fp32 a prefix near the total
-  // only resolves ulp(1) ~ 1.2e-7, more than a tail token behind a dominant one holds, and its rounding would both leave gaps
-  // between neighbouring chunks and line every chunk start up with the grid of fp32 targets (over-weighting each chunk's first
-  // token)
-  double incl = loc;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const double n = __shfl_up_sync(0xffffffffu, incl, o);
-    if ((threadIdx.x & 31) >= o) incl += n;
-  }
   if (threadIdx.x == 0) winner_s = -1;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 31) scan_s[threadIdx.x >> 5] = incl;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    double w = scan_s[threadIdx.x], wi = w;
-#pragma unroll
+  const int col = step_ptr ? step_ptr[0] : 0;                                // the output column; the draw's step when not per row
+  if (!greedy) {
+    // ---- max and partition function of z = logit / temperature
+    float m = -INFINITY;
+    visit([&](long long, float x, unsigned short) { if (x > m) m = x; });      // NaN never wins
+    m = block_max_f(m, red);
+    auto prob = [&](float x) { return x == x ? __expf((x - m) * inv_temp) : 0.f; };   // unnormalised; NaN logits get mass 0
+    unsigned kmax = 0;
+    visit([&](long long, float x, unsigned short bb) { if (x == x) { const unsigned k = key16(bb); if (k > kmax) kmax = k; } });
+    kmax = (unsigned)block_max_f((float)kmax, red);                            // keys < 2^16 are exact in fp32
+    auto mass_ge = [&](unsigned tau) {
+      float s = 0.f;
+      visit([&](long long, float x, unsigned short bb) { if (x == x && key16(bb) >= tau) s += prob(x); });
+      return block_sum_f(s, red);
+    };
+    auto count_ge = [&](unsigned tau) {
+      float c = 0.f;
+      visit([&](long long, float x, unsigned short bb) { if (x == x && key16(bb) >= tau) c += 1.f; });
+      return block_sum_f(c, red);                                              // counts <= 2^24 are exact in fp32
+    };
+    unsigned tau = 0;
+    if (top_k > 0 && (long long)top_k < vocab) {
+      unsigned lo = 0, hi = kmax + 1;                                          // count(>= lo) >= k holds, count(>= hi) = 0 does not
+      while (hi - lo > 1) {
+        const unsigned mid = lo + ((hi - lo) >> 1);
+        if (count_ge(mid) >= (float)top_k) lo = mid; else hi = mid;
+      }
+      tau = lo;
+    }
+    float mass = mass_ge(tau);
+    if (top_p > 0.f && top_p < 1.f) {
+      const float target = top_p * mass;
+      unsigned lo = tau, hi = kmax + 1;
+      while (hi - lo > 1) {
+        const unsigned mid = lo + ((hi - lo) >> 1);
+        if (mass_ge(mid) >= target) lo = mid; else hi = mid;
+      }
+      if (lo != tau) { tau = lo; mass = mass_ge(tau); }
+    }
+    // ---- inverse CDF in index order over the kept set
+    const int dstep = rp.draw_step ? rp.draw_step[b] : col;
+    const int dkey = rp.draw_key ? rp.draw_key[b] : b;
+    const unsigned long long h = splitmix64(seed ^ splitmix64(((unsigned long long)(unsigned)dstep << 32) | (unsigned)dkey));
+    const double u = (double)(h >> 40) * (1.0 / 16777216.0);                  // 24 random bits -> [0, 1)
+    float loc = 0.f;
+    visit([&](long long, float x, unsigned short bb) { if (x == x && key16(bb) >= tau) loc += prob(x); });
+    // block exclusive scan of the per-thread sums (threads own increasing index ranges), in fp64: in fp32 a prefix near the total
+    // only resolves ulp(1) ~ 1.2e-7, more than a tail token behind a dominant one holds, and its rounding would both leave gaps
+    // between neighbouring chunks and line every chunk start up with the grid of fp32 targets (over-weighting each chunk's first
+    // token)
+    double incl = loc;
+  #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-      const double n = __shfl_up_sync(0xffffffffu, wi, o);
-      if (threadIdx.x >= o) wi += n;
+      const double n = __shfl_up_sync(0xffffffffu, incl, o);
+      if ((threadIdx.x & 31) >= o) incl += n;
     }
-    scan_s[threadIdx.x] = wi - w;                                            // exclusive prefix of the warp totals
-    if (threadIdx.x == 31) total_s = wi;                                     // grand total (same summation tree every launch)
-  }
-  __syncthreads();
-  const double rel = u * total_s - (scan_s[threadIdx.x >> 5] + (incl - loc));   // where the draw lies from this chunk's start
-  // the owner of the draw: the last thread with mass that starts at or before it -- exactly one thread, however the prefixes
-  // of neighbouring chunks are rounded (NaN mass: none)
-  const float owner = block_max_f(loc > 0.f && rel >= 0.0 ? (float)threadIdx.x : -1.f, red);
-  if ((float)threadIdx.x == owner) {
-    // walk the chunk from 0: an fp32 sum started at the prefix (~ total) would not move for a tail token
-    const float t_loc = (float)rel;
-    float acc = 0.f;
-    int pick = -1, last = -1;
-    visit([&](long long i, float x, unsigned short bb) {
-      if (pick < 0 && x == x && key16(bb) >= tau) {
-        const float p = prob(x);
-        if (p > 0.f) {
-          acc += p;
-          last = (int)i;
-          if (t_loc < acc) pick = (int)i;
+    __syncthreads();
+    if ((threadIdx.x & 31) == 31) scan_s[threadIdx.x >> 5] = incl;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      double w = scan_s[threadIdx.x], wi = w;
+  #pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const double n = __shfl_up_sync(0xffffffffu, wi, o);
+        if (threadIdx.x >= o) wi += n;
+      }
+      scan_s[threadIdx.x] = wi - w;                                            // exclusive prefix of the warp totals
+      if (threadIdx.x == 31) total_s = wi;                                     // grand total (same summation tree every launch)
+    }
+    __syncthreads();
+    const double rel = u * total_s - (scan_s[threadIdx.x >> 5] + (incl - loc));   // where the draw lies from this chunk's start
+    // the owner of the draw: the last thread with mass that starts at or before it -- exactly one thread, however the prefixes
+    // of neighbouring chunks are rounded (NaN mass: none)
+    const float owner = block_max_f(loc > 0.f && rel >= 0.0 ? (float)threadIdx.x : -1.f, red);
+    if ((float)threadIdx.x == owner) {
+      // walk the chunk from 0: an fp32 sum started at the prefix (~ total) would not move for a tail token
+      const float t_loc = (float)rel;
+      float acc = 0.f;
+      int pick = -1, last = -1;
+      visit([&](long long i, float x, unsigned short bb) {
+        if (pick < 0 && x == x && key16(bb) >= tau) {
+          const float p = prob(x);
+          if (p > 0.f) {
+            acc += p;
+            last = (int)i;
+            if (t_loc < acc) pick = (int)i;
+          }
         }
-      }
-    });
-    winner_s = pick >= 0 ? pick : last;                                      // rounding left the walk short: the last token WITH mass
+      });
+      winner_s = pick >= 0 ? pick : last;                                      // rounding left the walk short: the last token WITH mass
+    }
   }
   __syncthreads();
+  int tok = winner_s;
+  if (tok < 0) tok = block_argmax(row, vocab, argmax_s);
   if (threadIdx.x == 0) {
-    int tok = winner_s;
-    if (tok < 0) {                                                           // no usable mass (total 0 or NaN: no finite logit, or +inf)
-      float best = -INFINITY;                                                // -> the first maximum, index 0 if none, as greedy
-      for (long long i = 0; i < vocab; ++i) {
-        const float x = DT<T>::to_f(row[i]);
-        if (x > best) { best = x; tok = (int)i; }
-      }
-      if (tok < 0) tok = 0;
-    }
-    if (out_tokens) out_tokens[(long long)b * out_ld + step] = tok;
+    if (rp.draw_step) rp.draw_step[b] += 1;                                  // tokens the row has produced, greedy ones included
+    if (out_tokens) out_tokens[(long long)b * out_ld + col] = tok;
     if (cur_ids) cur_ids[b] = tok;
     if (positions) {
       const int np = positions[b] + 1;
@@ -207,12 +263,30 @@ sample_advance_kernel(const T* __restrict__ logits, long long vocab, float inv_t
       const int done = atomicAdd(&step_ptr[1], 1) + 1;                       // step_ptr = {step, done-counter}
       if (done == (int)gridDim.x) {
         step_ptr[1] = 0;
-        step_ptr[0] = step + 1;
+        step_ptr[0] = col + 1;
       }
     }
   }
 }
 
+}  // namespace
+
+namespace {
+int launch_sample_advance(cts_ctx* ctx, const void* logits, long long vocab, int batch, float inv_temp, int top_k, float top_p,
+                          unsigned long long seed, const RowParams& rp, int* out_tokens, int out_ld, int* step_ptr, int* cur_ids,
+                          int* positions, int* seq_lens, int* slot_map, const int* page_table, int max_pages, int page_size, int dtype,
+                          void* stream) {
+  if (dtype == CTS_BF16) {
+    CTS_CUDA(ctx, launch_pdl(sample_advance_kernel<__nv_bfloat16>, dim3((unsigned)batch), dim3(kSaThreads), 0, (cudaStream_t)stream, 1,
+                             (const __nv_bfloat16*)logits, vocab, inv_temp, top_k, top_p, seed, rp, out_tokens, out_ld, step_ptr, cur_ids,
+                             positions, seq_lens, slot_map, page_table, max_pages, page_size));
+  } else {
+    CTS_CUDA(ctx, launch_pdl(sample_advance_kernel<__half>, dim3((unsigned)batch), dim3(kSaThreads), 0, (cudaStream_t)stream, 1,
+                             (const __half*)logits, vocab, inv_temp, top_k, top_p, seed, rp, out_tokens, out_ld, step_ptr, cur_ids, positions,
+                             seq_lens, slot_map, page_table, max_pages, page_size));
+  }
+  return CTS_OK;
+}
 }  // namespace
 
 extern "C" int cts_sample_advance(cts_ctx* ctx, const void* logits, long long vocab, int batch, float temperature, int top_k,
@@ -225,17 +299,25 @@ extern "C" int cts_sample_advance(cts_ctx* ctx, const void* logits, long long vo
   CTS_CHECK_ARG(ctx, dtype == CTS_BF16 || dtype == CTS_F16, "dtype");
   CTS_CHECK_ARG(ctx, page_size > 0 || slot_map == nullptr, "page_size");
   if (batch == 0) return CTS_OK;
-  const float inv_t = 1.0f / temperature;
-  if (dtype == CTS_BF16) {
-    CTS_CUDA(ctx, launch_pdl(sample_advance_kernel<__nv_bfloat16>, dim3((unsigned)batch), dim3(kSaThreads), 0, (cudaStream_t)stream, 1,
-                             (const __nv_bfloat16*)logits, vocab, inv_t, top_k, top_p, seed, out_tokens, out_ld, step_ptr, cur_ids,
-                             positions, seq_lens, slot_map, page_table, max_pages, page_size));
-  } else {
-    CTS_CUDA(ctx, launch_pdl(sample_advance_kernel<__half>, dim3((unsigned)batch), dim3(kSaThreads), 0, (cudaStream_t)stream, 1,
-                             (const __half*)logits, vocab, inv_t, top_k, top_p, seed, out_tokens, out_ld, step_ptr, cur_ids, positions,
-                             seq_lens, slot_map, page_table, max_pages, page_size));
-  }
-  return CTS_OK;
+  return launch_sample_advance(ctx, logits, vocab, batch, 1.0f / temperature, top_k, top_p, seed, RowParams{}, out_tokens, out_ld, step_ptr,
+                               cur_ids, positions, seq_lens, slot_map, page_table, max_pages, page_size, dtype, stream);
+}
+
+extern "C" int cts_sample_advance_rows(cts_ctx* ctx, const void* logits, long long vocab, int batch, const float* temperature,
+                                       const int* top_k, const float* top_p, const unsigned long long* seed, const int* draw_key,
+                                       int* draw_step, int* out_tokens, int out_ld, int* step_ptr, int* cur_ids, int* positions,
+                                       int* seq_lens, int* slot_map, const int* page_table, int max_pages, int page_size, int dtype,
+                                       void* stream) {
+  if (!ctx) return CTS_ERR_BAD_ARG;
+  CTS_CHECK_ARG(ctx, logits != nullptr && vocab > 0 && vocab <= (1LL << 24) && batch >= 0, "logits / vocab (<= 2^24) / batch");
+  CTS_CHECK_ARG(ctx, temperature != nullptr && top_k != nullptr && top_p != nullptr && seed != nullptr && draw_key != nullptr &&
+                     draw_step != nullptr, "null per-row temperature / top_k / top_p / seed / draw_key / draw_step");
+  CTS_CHECK_ARG(ctx, dtype == CTS_BF16 || dtype == CTS_F16, "dtype");
+  CTS_CHECK_ARG(ctx, page_size > 0 || slot_map == nullptr, "page_size");
+  if (batch == 0) return CTS_OK;
+  const RowParams rp{temperature, top_k, top_p, seed, draw_key, draw_step};
+  return launch_sample_advance(ctx, logits, vocab, batch, 1.f, 0, 1.f, 0ull, rp, out_tokens, out_ld, step_ptr, cur_ids, positions, seq_lens,
+                               slot_map, page_table, max_pages, page_size, dtype, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -12,12 +12,21 @@ between two replays by rewriting its slot's few integers:
   * free slots keep decoding a dummy sequence inside one reserved scratch page (their work is wasted, never wrong): the graph
     always runs at its full width, the price of never re-capturing.
 
-Greedy decoding; per-row arithmetic does not depend on the other rows, so a request produces the tokens a stand-alone
-``generate()`` call produces.  A request may carry vLLM's logits processors (chatts_b200.logit_proc), one parameter set per slot: a
-round in which some active slot uses them runs each step as the decode step without its advance followed by the stages of
-chatts_b200.token_pipeline (neutral and free slots are skipped); a round in which none does replays the plain graph.  Host logic only
-(torch copies of a few int32 per slot); every number comes from the kernels.
+Per-row arithmetic does not depend on the other rows, so a greedy request produces the tokens a stand-alone ``generate()`` call
+produces.  A request may sample (temperature, top_k, top_p, seed) and may carry vLLM's logits processors (chatts_b200.logit_proc), one
+parameter set per slot.  A round in which some active slot samples or uses processors runs each step as the decode step without its
+advance followed by the stages of chatts_b200.token_pipeline.  Their pick is cts_sample_advance_rows when some active slot samples
+(greedy slots, free ones included, take cts_greedy_advance's token, sampled ones their own draw) and cts_greedy_advance otherwise.  A
+round in which no active slot does either replays the plain graph.
+
+The draw rule: token i of a sampled request is drawn with u(seed, i, seed_row), the draw generate(seed=seed) makes for its row
+seed_row at step i.  It depends neither on the slot the request lands in nor on the round its steps fall in, so a seeded request is
+reproducible, and n requests for one prompt with one seed and seed_row = 0..n-1 give the n completions of
+``LLM.generate([prompt], SamplingParams(n=n, seed=seed))``.  An unseeded request draws a fresh seed, kept in ``Request.seed``.
+Host logic only (torch copies of a few numbers per slot); every number comes from the kernels.
 """
+import math
+import os
 from collections import deque
 from dataclasses import dataclass, field
 from types import SimpleNamespace
@@ -28,7 +37,7 @@ import torch
 from . import logit_proc as lpmodp
 from . import logprobs as lpmod
 from ._cabi import LOGPROBS_MAX_K
-from .token_pipeline import TokenPipeline, stop_ids
+from .token_pipeline import SamplingState, TokenPipeline, stop_ids
 
 
 @dataclass
@@ -48,6 +57,15 @@ class Request:
     logprobs: int = None               # top-k of the logprobs asked for (None: none)
     token_logprobs: list = field(default_factory=list)   # per token: (logprob, rank, top-k ids, top-k logprobs), as in generate()
     procs: lpmodp.Processors = None    # logits processors (None: none)
+    temperature: float = 0.0           # 0: greedy (top_k, top_p and seed unused)
+    top_k: int = 0                     # 0 or -1: off
+    top_p: float = 1.0
+    seed: int = None                   # the seed the request's tokens were drawn with (None for a greedy request)
+    seed_row: int = 0                  # the draw key: token i is u(seed, i, seed_row), generate(seed=seed)'s row seed_row at step i
+
+    @property
+    def samples(self):
+        return self.temperature > 0
 
 
 class ContinuousEngine:
@@ -74,14 +92,30 @@ class ContinuousEngine:
         self.occupancy = []                                # active slots per round (observability / tests)
         self._lpb = None                                   # logprob outputs of a round, made when a request first asks
         self._proc = None                                  # per-slot logits processors, made when a request first asks
+        self._samp = SamplingState(model.ctx, self.B, dev)  # per-slot sampling parameters (free slots: greedy)
 
     # ------------------------------------------------------------------------------------------ public
     def add_request(self, input_ids, series=None, max_new_tokens=16, eos_token_id=None, ignore_eos=False, logprobs=None,
                     presence_penalty=0.0, frequency_penalty=0.0, repetition_penalty=None, logit_bias=None, allowed_token_ids=None,
-                    min_tokens=None):
+                    min_tokens=None, temperature=0.0, top_k=0, top_p=1.0, seed=None, seed_row=0):
         """logprobs = k (0..20): every token's logprob and rank and the k most likely tokens, in Request.token_logprobs.
         presence_penalty, frequency_penalty, repetition_penalty, logit_bias, allowed_token_ids, min_tokens: the logits processors of
-        generate() (its min_new_tokens is min_tokens here), from the first token on; ValueError on a bad value."""
+        generate() (its min_new_tokens is min_tokens here), from the first token on.
+        temperature > 0 samples with top_k (0 or -1: off) and top_p in (0, 1]; token i is drawn with u(seed, i, seed_row), as
+        generate(seed=seed) draws its row seed_row at step i; seed None draws a fresh one (kept in Request.seed).  temperature 0 is
+        greedy and ignores the other three.  ValueError on a bad value, before anything is queued."""
+        temperature = float(temperature)
+        if not (math.isfinite(temperature) and temperature >= 0):
+            raise ValueError(f"temperature must be a finite number >= 0, got {temperature}")
+        top_k, top_p = int(top_k or 0), float(top_p)
+        if top_k < -1:
+            raise ValueError(f"top_k must be -1, 0 (off) or a positive count, got {top_k}")
+        if not 0 < top_p <= 1:
+            raise ValueError(f"top_p must be in (0, 1], got {top_p}")
+        if not 0 <= int(seed_row) < 1 << 31:
+            raise ValueError(f"seed_row must be in [0, 2^31), got {seed_row}")
+        if temperature > 0 and seed is None:
+            seed = int.from_bytes(os.urandom(8), "little")          # a fresh seed, kept so that the request can be replayed
         k = lpmod.check_k(logprobs, "logprobs")
         cfg = self.m.config
         procs = lpmodp.resolve(presence_penalty, frequency_penalty, repetition_penalty, logit_bias, allowed_token_ids, min_tokens,
@@ -91,6 +125,8 @@ class ContinuousEngine:
         ids = torch.as_tensor(input_ids, dtype=torch.long).reshape(-1)
         ts = series if series is not None else torch.zeros(0, 0, 1)
         r = Request(self._next, ids, ts, int(max_new_tokens), eos, ignore_eos, logprobs=k, procs=procs)
+        if temperature > 0:
+            r.temperature, r.top_k, r.top_p, r.seed, r.seed_row = temperature, top_k, top_p, int(seed), int(seed_row)
         self._next += 1
         self.waiting.append(r)
         return r.rid
@@ -194,10 +230,14 @@ class ContinuousEngine:
             prows = [i for i, r in enumerate(group) if r.procs is not None]
             if prows:
                 self._set_procs([group[i] for i in prows], [free[i] for i in prows])
+            for i, r in enumerate(group):
+                if r.samples:
+                    self._samp.set_rows([free[i]], r.temperature, r.top_k, r.top_p, r.seed, r.seed_row)
+            samples = any(r.samples for r in group)
             ks = [r.logprobs for r in group if r.logprobs is not None]
             lpb = lpmod.LogprobBuffers(m.ctx, g, 1, max(ks), m.config.vocab_size, dev) if ks else None
-            TokenPipeline(m.ctx, t, g, m.page_size, processors=self._proc if prows else None, slots=free[:g],
-                          logprobs=(lpb, max(ks)) if ks else None).step(logits)
+            TokenPipeline(m.ctx, t, g, m.page_size, sampling=self._samp if samples else None, processors=self._proc if prows else None,
+                          slots=free[:g], logprobs=(lpb, max(ks)) if ks else None).step(logits)
             first = t.out_tokens[:, 0].cpu().tolist()           # host read: the request's first token (and EOS check)
             if ks:
                 first_lp = lpb.host(1)
@@ -256,7 +296,9 @@ class ContinuousEngine:
         if ks and self._lpb is None:
             self._lpb = lpmod.LogprobBuffers(m.ctx, self.B, self.k, LOGPROBS_MAX_K, m.config.vocab_size, m.device)
         procs = any(r.procs is not None for r in self.active.values())
-        pipe = TokenPipeline(m.ctx, st, self.B, m.page_size, processors=self._proc if procs else None,
+        samples = any(r.samples for r in self.active.values())
+        pipe = TokenPipeline(m.ctx, st, self.B, m.page_size, sampling=self._samp if samples else None,
+                             processors=self._proc if procs else None,
                              logprobs=(self._lpb, max(ks)) if ks else None)          # logprobs: all slots at the largest k asked
         for _ in range(self.k):
             m._decode_step(st, sample=pipe.fused)
@@ -300,6 +342,8 @@ class ContinuousEngine:
         if r.slot >= 0:
             if r.procs is not None:
                 self._proc.reset_rows([r.slot])
+            if r.samples:
+                self._samp.reset_rows([r.slot])
             self.st.page_table[r.slot].fill_(self.scratch)
             self._reset_free([r.slot])
 

@@ -153,7 +153,7 @@ class Engine:
         """Iteration-level batching (engine.ContinuousEngine): requests join the static decode slots between graph replays and
         leave them at EOS / max_tokens; streaming requests get their new tokens after every round."""
         from .engine import ContinuousEngine
-        from .vllm_compat import CompletionOutput, RequestOutput, cut_at_stop, cut_at_stop_string_after, logprob_dict, tokens_before_stop_string
+        from .vllm_compat import RequestOutput, cut_at_stop, engine_completion
         llm = self.llm
         eng = ContinuousEngine(llm.model, steps_per_round=self.steps_per_round)
         jobs, sent = {}, {}
@@ -176,15 +176,8 @@ class Engine:
                     job.stream_q.put(None)
 
         def finish(job, r):
-            toks, fin = cut_at_stop(r.tokens, job.stop_ids, job.params.get("ignore_eos", False))
-            stops, mt = job.params.get("stop") or [], job.params.get("min_tokens", 0)
-            text, hit = cut_at_stop_string_after(llm.tokenizer, toks, stops, mt)
-            out = CompletionOutput(text, toks, "stop" if hit else fin)
-            if r.logprobs is not None:
-                keep = tokens_before_stop_string(llm.tokenizer, toks, stops, mt) if hit else len(toks)
-                out.logprobs = [logprob_dict(toks[j], *r.token_logprobs[j], llm.tokenizer) for j in range(keep)]
-                out.cumulative_logprob = float(sum(r.token_logprobs[j][0] for j in range(keep)))
-            return out
+            return engine_completion(llm.tokenizer, r, job.stop_ids, job.params.get("ignore_eos", False), job.params.get("stop") or [],
+                                     job.params.get("min_tokens", 0))
 
         while not self.stop:
             if not eng.has_work():

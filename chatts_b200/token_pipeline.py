@@ -4,8 +4,9 @@ buffer [rows, >= V].  Each step runs, on the device and with no host round trip:
   1. the structured-output mask: the logits of the tokens a row's automaton refuses become -inf (cts_struct_mask_apply);
   2. the logits processors (chatts_b200.logit_proc states their order): cts_rep_penalty_apply when repetition_penalty is the only one
      set, cts_logit_proc_apply otherwise;
-  3. the pick and advance of every row's decode state: cts_greedy_advance, or cts_sample_advance with temperature / top-k / top-p and a
-     draw that is a function of (seed, step, row);
+  3. the pick and advance of every row's decode state: cts_greedy_advance; cts_sample_advance with temperature / top-k / top-p and a
+     draw that is a function of (seed, step, row), one parameter set for every row (generate()); or cts_sample_advance_rows with each
+     row's own parameters and a draw that is a function of (seed, draw step, draw key) of the row (SamplingState: the engine's slots);
   4. the processor update (the new token's occurrence bit and count) and the automaton's walk over the new token;
   5. the logprobs (cts_logprobs) of the logits the token was picked from, at the column the advance wrote.
 
@@ -134,11 +135,49 @@ def generate_processors(ctx, procs, ids_cpu, am_cpu, stops, vocab, n_pos, device
     return state
 
 
+class SamplingState:
+    """Per-row sampling parameters on the device for ``rows`` rows (the continuous engine's slots), read by cts_sample_advance_rows:
+    temperature (<= 0: greedy), top_k (<= 0: off), top_p, seed, and the draw of a row's token i, u(seed, draw_step, draw_key) with
+    draw_step = i: the kernel adds 1 per token.  A row that was never set, or was reset, is greedy."""
+
+    def __init__(self, ctx, rows, device):
+        self.ctx, self.rows, self.dev = ctx, int(rows), device
+        f32, i32 = dict(dtype=torch.float32, device=device), dict(dtype=torch.int32, device=device)
+        self.temperature, self.top_p = torch.zeros(rows, **f32), torch.ones(rows, **f32)
+        self.top_k, self.draw_key, self.draw_step = torch.zeros(rows, **i32), torch.zeros(rows, **i32), torch.zeros(rows, **i32)
+        self.seed = torch.zeros(rows, dtype=torch.int64, device=device)
+
+    def set_rows(self, idx, temperature, top_k, top_p, seed, draw_key):
+        """Rows ``idx`` (list of ints) start a request with these parameters; its first token is draw 0."""
+        ix = torch.as_tensor(idx, dtype=torch.long, device=self.dev)
+        self.temperature[ix], self.top_k[ix], self.top_p[ix] = float(temperature), int(top_k), float(top_p)
+        s = int(seed) & ((1 << 64) - 1)
+        self.seed[ix] = s - (1 << 64) if s >= 1 << 63 else s          # stored as int64, read as uint64
+        self.draw_key[ix], self.draw_step[ix] = int(draw_key), 0
+
+    def reset_rows(self, idx):
+        self.set_rows(idx, 0.0, 0, 1.0, 0, 0)
+
+    def advance(self, logits, n, out_tokens, step_ptr, cur_ids, positions, seq_lens, slot_map, page_table, page_size, slots=None):
+        """Pick and advance logits rows [0, n); ``slots``: logits row i uses state row slots[i] (default: row i)."""
+        adv = (out_tokens, step_ptr, cur_ids, positions, seq_lens, slot_map, page_table, page_size)
+        if slots is None:
+            self.ctx.sample_advance_rows(logits, n, self.temperature, self.top_k, self.top_p, self.seed, self.draw_key, self.draw_step,
+                                         *adv)
+            return
+        ix = torch.as_tensor(slots, dtype=torch.long, device=self.dev)[:n]
+        step = self.draw_step[ix]
+        self.ctx.sample_advance_rows(logits, n, self.temperature[ix], self.top_k[ix], self.top_p[ix], self.seed[ix], self.draw_key[ix],
+                                     step, *adv)
+        self.draw_step[ix] = step
+
+
 class TokenPipeline:
     """The stages above for ``rows`` rows of one logits buffer.  ``st`` holds the advance buffers (out_tokens, step_ptr, cur_ids,
     positions, seq_lens, slot_map, page_table) and, after a decode step, its ``full_logits``.  sampling: (temperature, top_k, top_p,
-    seed), None for greedy; automaton: (structured.DeviceAutomaton, int32 state [rows]); processors: a LogitProcState or a
-    RepetitionPenaltyState, whose row slots[i] belongs to logits row i when ``slots`` is given; logprobs: (LogprobBuffers, k)."""
+    seed) for every row, or a SamplingState, or None for greedy; automaton: (structured.DeviceAutomaton, int32 state [rows]);
+    processors: a LogitProcState or a RepetitionPenaltyState; when ``slots`` is given, row slots[i] of the processors and of a
+    SamplingState belongs to logits row i; logprobs: (LogprobBuffers, k)."""
 
     def __init__(self, ctx, st, rows, page_size, sampling=None, automaton=None, processors=None, slots=None, logprobs=None):
         self.ctx, self.st, self.rows, self.page_size, self.sampling, self.processors = ctx, st, rows, page_size, sampling, processors
@@ -163,6 +202,8 @@ class TokenPipeline:
             adv = (st.out_tokens, st.step_ptr, st.cur_ids, st.positions, st.seq_lens, st.slot_map, st.page_table, self.page_size)
             if self.sampling is None:
                 c.greedy_advance(lg, n, *adv)
+            elif isinstance(self.sampling, SamplingState):
+                self.sampling.advance(lg, n, *adv, *self.proc_slots)
             else:
                 c.sample_advance(lg, n, *self.sampling, *adv)
             if self.processors is not None:

@@ -137,6 +137,20 @@ def cut_at_stop(tokens, stop_ids, ignore_eos=False):
     return toks, "length"
 
 
+def engine_completion(tokenizer, r, stop_ids, ignore_eos=False, stops=(), min_tokens=0):
+    """The CompletionOutput of a finished continuous-engine Request (engine.Request): the tokens before the first stop id, the text
+    cut before a stop string that counts after min_tokens, the logprob dicts and cumulative_logprob of the tokens that text came
+    from (when the request asked for logprobs), and the finish_reason."""
+    toks, fin = cut_at_stop(r.tokens, stop_ids, ignore_eos)
+    text, hit = cut_at_stop_string_after(tokenizer, toks, stops, min_tokens)
+    out = CompletionOutput(text, toks, "stop" if hit else fin)
+    if r.logprobs is not None:
+        keep = tokens_before_stop_string(tokenizer, toks, stops, min_tokens) if hit else len(toks)
+        out.logprobs = [logprob_dict(toks[j], *r.token_logprobs[j], tokenizer) for j in range(keep)]
+        out.cumulative_logprob = float(sum(r.token_logprobs[j][0] for j in range(keep)))
+    return out
+
+
 def decode_text(tokenizer, tokens):
     """tokenizer.decode(..., skip_special_tokens=True) (inference_tsmllm_deepspeed.py:104-106), for tokenizers that take the flag."""
     try:
@@ -313,15 +327,25 @@ class LLM:
             pass
 
     def generate(self, inputs, sampling_params=None, use_tqdm=False, streamer=None):
+        """sampling_params: one SamplingParams for every prompt, or a list of one per prompt (as vLLM takes it).  A list whose
+        entries differ runs the prompts through the continuous engine (_generate_per_prompt); an all-equal list is the single
+        SamplingParams."""
+        if isinstance(inputs, (dict, str)):
+            inputs = [inputs]
+        # plain strings are text-only prompts (llm_utils.py:127 passes a list of str to the same call)
+        inputs = [{"prompt": r} if isinstance(r, str) else r for r in inputs]
+        if isinstance(sampling_params, (list, tuple)):
+            sps = [p or SamplingParams() for p in sampling_params]
+            if len(sps) != len(inputs):
+                raise ValueError(f"{len(sps)} SamplingParams for {len(inputs)} prompts: give one, or one per prompt")
+            if any(p != sps[0] for p in sps[1:]):
+                return self._generate_per_prompt(inputs, sps, streamer)
+            sampling_params = sps[0] if sps else None
         sp = sampling_params or SamplingParams()
         if (sp.logprobs is not None or sp.prompt_logprobs is not None) and self.model.tp_size > 1:
             raise ValueError("logprobs / prompt_logprobs are single-GPU only (tensor_parallel_size must be 1)")
         if sp.structured_outputs is not None and self.model.tp_size > 1:
             raise ValueError("structured_outputs are single-GPU only (tensor_parallel_size must be 1)")
-        if isinstance(inputs, (dict, str)):
-            inputs = [inputs]
-        # plain strings are text-only prompts (llm_utils.py:127 passes a list of str to the same call)
-        inputs = [{"prompt": r} if isinstance(r, str) else r for r in inputs]
         n = max(1, int(sp.n))
         if n > 1:
             # n completions per request = n copies of the request in the batch, each row with its own draw
@@ -330,6 +354,58 @@ class LLM:
             return [RequestOutput(inputs[i]["prompt"], [flat[i * n + j].outputs[0] for j in range(n)], flat[i * n].num_cached_tokens,
                                   flat[i * n].prompt_logprobs) for i in range(len(inputs))]
         return self._generate(inputs, sp, streamer)
+
+    def _generate_per_prompt(self, inputs, sps, streamer=None):
+        """Prompts with different SamplingParams, through a ContinuousEngine over model.max_batch slots: each prompt keeps its own
+        max_tokens, stop ids and strings, ignore_eos, n, logprobs, processors, temperature, top_k, top_p and seed.  Copy j of a
+        prompt's n is drawn with seed_row = j, so a seeded prompt gets what LLM.generate([prompt], its SamplingParams) gives.
+        Outputs come back in prompt order."""
+        from .engine import ContinuousEngine
+        if streamer is not None:
+            raise ValueError("a streamer needs one SamplingParams for every prompt")
+        if self.model.tp_size > 1:
+            raise ValueError("per-prompt SamplingParams are single-GPU only (tensor_parallel_size must be 1)")
+        for sp in sps:
+            if sp.structured_outputs is not None:
+                raise ValueError("structured_outputs need one SamplingParams for every prompt")
+            if sp.prompt_logprobs is not None:
+                raise ValueError("prompt_logprobs need one SamplingParams for every prompt")
+        gd = getattr(self.model, "generation_defaults", None) or {}
+        encs = []
+        for req in inputs:
+            ts = (req.get("multi_modal_data") or {}).get("timeseries", [])
+            if len(ts) > self.limit:
+                raise ValueError(f"at most {self.limit} time series per prompt")
+            for t in ts:
+                if not isinstance(t, (list, np.ndarray, torch.Tensor)):
+                    raise TypeError(f"Unsupported time series type: {type(t)}")
+            encs.append(self.processor(text=[req["prompt"]], timeseries=list(ts), padding=True, return_tensors="pt"))
+        eng = ContinuousEngine(self.model)
+        try:
+            rids = []
+            for enc, sp in zip(encs, sps):
+                stop_ids = eos_ids(self.model.config, sp.stop_token_ids, gd.get("eos_token_id"))
+                rep = sp.repetition_penalty if sp.repetition_penalty not in (None, 1.0) else gd.get("repetition_penalty")
+                rids.append([eng.add_request(enc["input_ids"][0], enc["timeseries"], max_new_tokens=sp.max_tokens, eos_token_id=stop_ids,
+                                             ignore_eos=sp.ignore_eos, logprobs=sp.logprobs, presence_penalty=sp.presence_penalty,
+                                             frequency_penalty=sp.frequency_penalty, repetition_penalty=rep, logit_bias=sp.logit_bias,
+                                             allowed_token_ids=sp.allowed_token_ids, min_tokens=sp.min_tokens, temperature=sp.temperature,
+                                             top_k=sp.top_k if sp.top_k and sp.top_k > 0 else 0, top_p=sp.top_p, seed=sp.seed, seed_row=j)
+                             for j in range(max(1, int(sp.n)))])
+            done = {r.rid: r for r in eng.run()}
+        finally:
+            eng.close()
+        outs = []
+        for req, sp, ids in zip(inputs, sps, rids):
+            reqs = [done[i] for i in ids]
+            err = next((r.error for r in reqs if r.error is not None), None)
+            if err is not None:
+                raise err
+            stops = [sp.stop] if isinstance(sp.stop, str) else list(sp.stop or [])
+            stop_ids = eos_ids(self.model.config, sp.stop_token_ids, gd.get("eos_token_id"))
+            outs.append(RequestOutput(req["prompt"], [engine_completion(self.tokenizer, r, stop_ids, sp.ignore_eos, stops, sp.min_tokens)
+                                                      for r in reqs], reqs[0].cached_positions))
+        return outs
 
     def _generate(self, inputs, sp, streamer=None):
         if self._tp_driver:                                  # the spawned ranks run the same call on their shards

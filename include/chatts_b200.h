@@ -218,6 +218,19 @@ int cts_sample_advance(cts_ctx* ctx, const void* logits, long long vocab, int ba
                        unsigned long long seed, int* out_tokens, int out_ld, int* step_ptr, int* cur_ids, int* positions,
                        int* seq_lens, int* slot_map, const int* page_table, int max_pages, int page_size, int dtype, void* stream);
 
+/* K13 with per-row parameters (the continuous engine's slots): the same kernel as cts_sample_advance, every parameter read per row.
+ *   temperature float[batch], top_k int[batch] (<= 0: off), top_p float[batch] (outside (0, 1): off), seed uint64[batch],
+ *   draw_key int[batch], draw_step int[batch]: all non-null.
+ *   Row b with !(temperature[b] > 0) is greedy: exactly cts_greedy_advance's token (first maximum, NaN never wins, 0 when no value
+ *   exceeds -inf).  Any other row is drawn as cts_sample_advance draws, with its own top_k / top_p and the uniform
+ *   u(seed[b], draw_step[b], draw_key[b]) in place of u(seed, step_ptr[0], b).  draw_step[b] += 1 for every row, greedy ones included.
+ *   out_tokens (column step_ptr[0]), step_ptr, cur_ids, positions, seq_lens and slot_map advance as in cts_sample_advance.
+ *   With equal parameters, draw_key[b] = b and draw_step[b] = step_ptr[0], the result is cts_sample_advance's, bit for bit. */
+int cts_sample_advance_rows(cts_ctx* ctx, const void* logits, long long vocab, int batch, const float* temperature, const int* top_k,
+                            const float* top_p, const unsigned long long* seed, const int* draw_key, int* draw_step, int* out_tokens,
+                            int out_ld, int* step_ptr, int* cur_ids, int* positions, int* seq_lens, int* slot_map, const int* page_table,
+                            int max_pages, int page_size, int dtype, void* stream);
+
 /* Log probabilities of `rows` rows of 16-bit logits [rows, ld] (vLLM's raw logprobs), in fp32 from the stored values:
  *   lse = m + log sum_i exp(x_i - m);  chosen_logprob = x_c - lse;  chosen_rank = 1 + #{i : x_i > x_c};
  *   the k (0..20) largest entries as (id, x_i - lse), by value descending, equal values by the smaller id.

@@ -159,6 +159,10 @@ SELECT = {
     # the sampler against its exact distribution: the far tail behind a dominant token (400 draws per case), the threshold edges,
     # draw-for-draw agreement, and the refusal masks chained into it (the full-row chi-square and the graph replay need a GPU)
     "test_gpu_zz_n_sampling_dist.py": "not whole_row and not repeated_launches and not graph_replay",
+    # the per-row sampler: uniform parameters against cts_sample_advance, mixed rows in one launch and the refusal chains at the
+    # small vocabularies, and the engine on the tiny model (the chi-square and the graph replay need a GPU)
+    "test_gpu_zz_o_sampling_rows.py": "(far_tail and bf16) or edges or (vocab_sizes and (1000 or 1003 or 8193)) "
+                                      "or (mixed and (1000 or 8193)) or refused or engine",
 }
 
 # --quick: a subset that finishes in about a minute (what tests/test_shim_kernels.py runs inside the CPU suite)
