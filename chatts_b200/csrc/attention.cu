@@ -373,9 +373,10 @@ attn_prefill_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid
   for (int j = 0; j < ntiles; ++j) {
     const int s = j % kWgStages;
     mbar_wait(&full_bar[s], (uint32_t)(j / kWgStages) & 1u);
-    if constexpr (PAGED) {
-      // Keys at or past kv_len get p = 0, but their V rows hold whatever the cache holds there (recycled pages are never cleared,
-      // page-table entries past the sequence point anywhere) and 0 * NaN = NaN: those rows are zeroed before the P V MMA.
+    {
+      // Keys at or past kv_len get p = 0, but their V rows hold whatever sits there and 0 * NaN = NaN: in the paged cache recycled
+      // pages are never cleared and page-table entries past the sequence point anywhere; in packed Q / K / V the rows past the last
+      // sequence (up to the buffer's row bound) hold what an earlier, longer batch left.  Those rows are zeroed before the P V MMA.
       const int nz = (j + 1) * kWgKV - kv_len;           // CTA-uniform
       if (nz > 0) {
         uint8_t* vs = kv_s + (size_t)s * kWgStageBytes + 2 * kWgHalf;
